@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Headline benchmark: offline serving throughput (output tokens/s) of Qwen3-8B bf16 with TP=N on N
-B200s, on synthetic ShareGPT-shaped requests with random-init weights (BASELINE.json metric;
+H100s, on synthetic ShareGPT-shaped requests with random-init weights (BASELINE.json metric;
 workload definition = the reference's benchmarks/benchmark_throughput.py: all requests submitted at
 t=0, prompt <= 1024, prompt+output <= 2048, greedy, ignore_eos).
 
@@ -13,7 +13,9 @@ the batch arrays from pinned memory and the D2H read of the sampled tokens.
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 \
         --master-port 29500 bench.py --gpus 8 --steps 3 --warmup 3
 
-Prints ONE JSON line on rank 0.
+Prints ONE JSON line on rank 0. `--dump-outputs DIR` also writes the token ids the last timed pass generated
+(DIR/output_token_ids.npy, every request's output concatenated in request order, and DIR/output_lens.npy), so two
+builds can be compared output for output: with the same arguments the inputs and weights are identical.
 """
 import argparse
 import json
@@ -44,8 +46,10 @@ def parse():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--model", default="preset:qwen3-8b")
-    ap.add_argument("--num-prompts", type=int, default=1000,
-                    help="the reference harness default (benchmarks/benchmark_throughput.py:359)")
+    ap.add_argument("--num-prompts", type=int, default=500,
+                    help="requests per pass. 500 keep every request's KV resident on one 80 GB H100 next to the 16 GB "
+                         "of weights (about 230 k tokens at 144 KB each); the reference harness's default of 1000 "
+                         "(benchmarks/benchmark_throughput.py:359) needs about 67 GB of KV")
     ap.add_argument("--maxp", type=int, default=4096)
     ap.add_argument("--maxd", type=int, default=1024)
     ap.add_argument("--max-cuda-graph-bs", type=int, default=512)
@@ -61,6 +65,8 @@ def parse():
                     help="lookahead decode scheduling (engine default; --no-async-schedule for the synchronous loop)")
     ap.add_argument("--disable-cuda-graph", action="store_true", help="debugging: every step runs eagerly")
     ap.add_argument("--num-gpu-pages", type=int, default=None, help="debugging: fixed KV pool size (pages)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the outputs of the last timed pass as .npy files into DIR")
     ap.add_argument("--fixed-prompts", action="store_true",
                     help="re-use the same token ids in every pass (with prefix caching the prompts of later passes "
                          "would then be served from the cache: NOT the benchmark; for debugging only)")
@@ -162,7 +168,7 @@ def synth_requests(n, vocab, seed, pass_idx=0):
 class ClockSampler(threading.Thread):
     QUERY = "index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active," \
             "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown," \
-            "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
+            "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,power.limit,name"
 
     def __init__(self, gpu_index=0):
         super().__init__(daemon=True)
@@ -184,7 +190,7 @@ class ClockSampler(threading.Thread):
             self.proc.terminate()
 
     def summary(self):
-        sm, mx, reasons = [], 0, set()
+        sm, mx, reasons, plim, gpu = [], 0, set(), None, None
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
         for r in self.rows:
             try:
@@ -193,13 +199,15 @@ class ClockSampler(threading.Thread):
                 for nme, v in zip(names, r[5:9]):
                     if v.lower().startswith("active"):
                         reasons.add(nme)
+                plim, gpu = float(r[9]), r[10]
             except Exception:  # noqa: BLE001
                 continue
         sm.sort()
         # median over samples under load (upper half of the distribution)
         load = sm[len(sm) // 2:] if sm else []
         med = load[len(load) // 2] if load else None
-        return {"sm_mhz": med, "sm_max_mhz": mx or None, "reasons": sorted(reasons), "samples": len(sm)}
+        return {"gpu": gpu, "power_limit_w": plim, "sm_mhz": med, "sm_max_mhz": mx or None,
+                "reasons": sorted(reasons), "samples": len(sm)}
 
 
 def main():
@@ -256,7 +264,7 @@ def main():
     runner = llm.worker.runner
 
     # token ids of every pass prepared up front (host work outside the timed region; the reference arm does the same)
-    n_pass = args.warmup + 2 * args.steps
+    n_pass = args.warmup + args.steps
     pass_prompts = [prompts if (args.fixed_prompts or i == 0) else synth_requests(args.num_prompts, vocab, args.seed, i)[0]
                     for i in range(n_pass)]
     if cpu_selftest:
@@ -277,10 +285,9 @@ def main():
     for _ in range(args.warmup):
         one_pass()
 
-    # ---- region A: K passes through the public API (LLM.generate: every iteration copies its batch arrays
+    # ---- timed region: K passes through the public API (LLM.generate: every iteration copies its batch arrays
     # host->device from pinned memory and reads the sampled tokens back), bracketed by barrier + sync and timed with
-    # CUDA events on the launching stream -> `value`. Region B below repeats K passes under the host's wall clock
-    # -> `e2e` (an independent measurement, not the same bracket read with a second clock).
+    # CUDA events on the launching stream -> `value`, and with the host's wall clock -> `e2e`.
     sampler = ClockSampler(int(os.environ.get("LOCAL_RANK", "0"))) if rank == 0 else None
     if sampler:
         sampler.start()
@@ -289,8 +296,9 @@ def main():
     stats0 = dict(runner.stats)
     launches0 = sm100.launches()
     barrier()
+    t0 = time.perf_counter()
     if cpu_selftest:
-        th0 = time.perf_counter()
+        th0 = t0
     else:
         ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         ev0.record()
@@ -300,18 +308,12 @@ def main():
     if not cpu_selftest:
         ev1.record()
     barrier()
+    wall_s = time.perf_counter() - t0
     dev_ms = (time.perf_counter() - th0) * 1e3 if cpu_selftest else ev0.elapsed_time(ev1)
     busy_ms = runner.gpu_busy_ms()
     runner.time_steps = False
     stats1 = dict(runner.stats)
     launches = (sm100.launches() - launches0) + (stats1["graph_kernel_launches"] - stats0["graph_kernel_launches"])
-    # ---- region B: end to end through the public API, wall clock ----
-    barrier()
-    t0 = time.perf_counter()
-    for _ in range(args.steps):
-        seqs = one_pass()
-    barrier()
-    wall_s = time.perf_counter() - t0
     if sampler:
         sampler.stop()
     if world > 1:
@@ -329,7 +331,9 @@ def main():
         except Exception:  # noqa: BLE001
             pass
         eng_steps = stats1["steps"] - stats0["steps"]
-        # request latencies of the last end-to-end pass (all requests arrive together at t0: offline workload)
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, seqs)
+        # request latencies of the last timed pass (all requests arrive together at t0: offline workload)
         lat = None
         try:
             ttft = sorted((q.first_token_time - q.arrival_time) * 1e3 for q in seqs if q.first_token_time)
@@ -337,7 +341,7 @@ def main():
                           for q in seqs if q.first_token_time and q.finish_time and q.num_output_tokens > 1)
             lat = {"p50_ttft_ms": round(ttft[len(ttft) // 2], 1), "p99_ttft_ms": round(ttft[int(len(ttft) * 0.99)], 1),
                    "p50_tpot_ms": round(tpot[len(tpot) // 2], 2), "p99_tpot_ms": round(tpot[int(len(tpot) * 0.99)], 2),
-                   "arrival": "all requests at t0 (offline batch)", "source": "last end-to-end pass"}
+                   "arrival": "all requests at t0 (offline batch)", "source": "last timed pass"}
         except Exception:  # noqa: BLE001
             pass
         out = {
@@ -376,6 +380,16 @@ def main():
     sys.stderr.flush()
     teardown(llm, world)
     return 0
+
+
+def dump_outputs(out_dir, seqs):
+    """The arrays a caller of LLM.generate receives from the last timed pass: every request's generated token ids
+    (float64, exact for any vocabulary), concatenated in request order, and the per-request output lengths."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    outs = [list(q.token_ids[q.prompt_len:]) for q in seqs]
+    np.save(os.path.join(out_dir, "output_token_ids.npy"), np.asarray([t for o in outs for t in o], dtype=np.float64))
+    np.save(os.path.join(out_dir, "output_lens.npy"), np.asarray([len(o) for o in outs], dtype=np.float64))
 
 
 def teardown(llm, world):

@@ -1,4 +1,4 @@
-"""Micro-benchmarks of the sm_100a kernels against their rooflines (CUDA-event timing, L2 flushed
+"""Micro-benchmarks of the sm_90a kernels against their rooflines (CUDA-event timing, L2 flushed
 between iterations). Prints one JSON line per case; cuBLAS / flash-attn numbers are printed only
 as context for the same shapes.
 
@@ -104,8 +104,8 @@ def bench_attn():
         scale = 1 / math.sqrt(d)
         flops = 4.0 * b * hq * d * ql * ql / 2
         variants = [("mma.sync", False, 0)]
-        if os.environ.get("KB_ATTN_TC", "0") == "1":      # opt-in tcgen05 kernel, both KV tile sizes
-            variants += [("tcgen05", True, 128), ("tcgen05", True, 64)]
+        if os.environ.get("KB_ATTN_TC", "0") == "1":      # wgmma kernel, both KV tile sizes
+            variants += [("wgmma", True, 128), ("wgmma", True, 64)]
         for name, tc, kvt in variants:
             sm100.ATTN_TC, sm100.ATTN_TC_KV = tc, (kvt or 128)
             ms = timeit(lambda: sm100.paged_attention(q, kc, vc, bt, sl, qsl, scale, hq, d, 0, b, ql, ql, out=out),

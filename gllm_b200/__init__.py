@@ -1,4 +1,4 @@
-"""gllm_b200 — a Blackwell (B200 / sm_100a) native LLM serving engine.
+"""gllm_b200 — a Hopper (H100 / sm_90a) native LLM serving engine.
 
 Public API mirrors the reference engine (`gllm/__init__.py:1-3`):
 

@@ -1,4 +1,4 @@
-"""In-tree build of the sm_100a kernel library (`gllm_b200/_C/libgllm_b200.so`).
+"""In-tree build of the sm_90a kernel library (`gllm_b200/_C/libgllm_b200.so`).
 
 Plain `nvcc` -> one shared object with a C ABI (loaded through ctypes in
 `gllm_b200.ops.lib`). No torch headers are needed, so a full rebuild takes
@@ -20,7 +20,7 @@ OUT_DIR = os.path.join(ROOT, "_C")
 LIB_PATH = os.path.join(OUT_DIR, "libgllm_b200.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "--use_fast_math",
     "-Xcompiler", "-fPIC",

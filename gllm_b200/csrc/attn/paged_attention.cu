@@ -1,8 +1,8 @@
-// Paged flash attention for sm_100a (prefill with chunked-prefill/prefix offsets, and
+// Paged flash attention for sm_90a (prefill with chunked-prefill/prefix offsets, and
 // split-KV decode), replacing the reference's `flash_attn_varlen_func` call on the paged cache
-// (gllm/layers/attention.py:49-61; FA2 sm_80 binary on Blackwell, SURVEY §2.3 K1).
+// (gllm/layers/attention.py:49-61; FA2 sm_80 binary, SURVEY §2.3 K1).
 //
-// Data movement is Blackwell-native: every KV page is fetched by one TMA tensor copy
+// Data movement is Hopper-native: every KV page is fetched by one TMA tensor copy
 // (cp.async.bulk.tensor.3d, 128-byte swizzle) into an mbarrier-synchronised multi-stage ring
 // filled by a dedicated producer warp; math warps consume the swizzled tiles with ldmatrix and
 // run the online-softmax recurrence on tensor cores (m16n8k16, fp32 accumulate).

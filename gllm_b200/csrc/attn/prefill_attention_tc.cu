@@ -1,38 +1,29 @@
-// tcgen05 / TMEM paged flash attention for prefill (chunked-prefill and prefix offsets included): the
-// Blackwell-native successor of the mma.sync prefill kernel in paged_attention.cu (same arguments, same
-// paged KV cache; reference call site: gllm/layers/attention.py:49-61, flash_attn_varlen_func on the paged cache).
-//
-// OPT-IN (GLLM_ATTN_TC=1, see ops/sm100.py) until it has been validated on hardware: written and compiled this
-// round on a GPU-less box. tests/test_kernels_gpu.py::test_prefill_attention_tc runs it against the fp32 oracle
-// when the switch is set.
+// wgmma paged flash attention for prefill (chunked-prefill and prefix offsets included): the tensor-core
+// successor of the mma.sync prefill kernel in paged_attention.cu (same arguments, same paged KV cache;
+// reference call site: gllm/layers/attention.py:49-61, flash_attn_varlen_func on the paged cache).
+// GLLM_ATTN_TC=0 (ops/sm100.py) selects the mma.sync kernel instead.
 //
 // One CTA = 128 query rows (128/GP tokens x GP heads that share one KV head, GQA-packed like the mma.sync kernel)
 // x the causal prefix of one sequence, walked in tiles of KV keys:
 //
-//   warp 4 (1 thread)  TMA producer : page boxes [page_size][64] of K and V -> smem tiles [D/64][KV][64] (SW128)
-//   warp 5 (1 thread)  MMA issuer   : S_b = Q K^T  (tcgen05.mma, A = Q smem K-major, B = K tile K-major, D in TMEM)
-//                                     O  += P_b V  (A = P smem K-major, B = V tile **MN-major**, D in TMEM)
-//   warps 0-3          softmax      : one query row per thread (tcgen05.ld 32x32b: a thread owns a TMEM lane):
-//                                     row max / exp2 / row sum without shuffles, P (bf16) -> smem as the A operand
-//                                     of the PV product, O rescaled in TMEM only when a row max moved
-//
-// S and P are double buffered, so QK^T of tile j+1 runs under the softmax of tile j and PV_j under softmax j+1.
-// TMEM columns: S0 [0, KV) | S1 [KV, 2KV) | O [2KV, 2KV + D).
+//   warpgroup 0 (1 thread)  TMA producer : page boxes [page_size][64] of K and V -> smem tiles [D/64][KV][64] (SW128)
+//   warpgroups 1-2          64 query rows each:
+//                             S = Q K^T   wgmma, A = Q smem K-major, B = K tile K-major, S in registers
+//                             softmax     row max / exp2 / row sum in registers (a row lives in 4 lanes of a quad)
+//                             O += P V    wgmma, A = P from registers (the S fragment converted to bf16 in place),
+//                                         B = V tile **MN-major**, O in registers
 //
 // The V operand: the cache stores V as [key][d] (d contiguous), i.e. the contraction dimension (keys) runs along
-// ROWS of the tile. That is the MN-major canonical layout of the UMMA shared-memory descriptor
+// ROWS of the tile. That is the MN-major canonical layout of the wgmma shared-memory descriptor
 //     SW128, MN-major, in 16-byte units: ((8, n), (8, k)) : ((1, LBO), (8, SBO))
 // -> 64 d-values (128 B) contiguous, next 64 d-values LBO bytes away (= one [KV][64] slab), 8 keys are 8
 // consecutive 128-byte rows, the next 8 keys SBO = 1024 B away; a K = 16 step advances the start address by 2048 B.
-// The four fields can be overridden at run time (GLLM_ATTN_TC_V = "lbo16,sbo16,kadv16,split_n") so that a
-// mismatch with the hardware can be bisected in one GPU call (benchmarks/umma_mn_sweep.py sweeps the same fields).
 #include "attn_common.cuh"
 
 namespace b200 {
 
-static constexpr int kTcRows = 128;                      // query rows per CTA (UMMA M)
-static constexpr int kTcSoftmaxWarps = 4;
-static constexpr int kTcThreads = (kTcSoftmaxWarps + 2) * 32;
+static constexpr int kTcRows = 128;                      // query rows per CTA (2 x wgmma M)
+static constexpr int kTcThreads = 384;
 
 struct TcAttnParams {
   const __nv_bfloat16* q;
@@ -43,7 +34,6 @@ struct TcAttnParams {
   const int32_t* q_start;
   int max_blocks, Hq, Hkv, G, GP, page_size, seq_offset;
   float scale_log2;
-  uint32_t v_lbo16, v_sbo16, v_kadv16, v_split_n;   // MN-major V descriptor fields (16-byte units)
 };
 
 template <int D, int KV>
@@ -51,42 +41,13 @@ struct TcSmem {
   static constexpr int kQBytes = kTcRows * D * 2;
   static constexpr int kTileBytes = KV * D * 2;            // one K (or V) tile
   static constexpr int kStageBytes = 2 * kTileBytes;
-  static constexpr int kPBytes = kTcRows * KV * 2;
-  static constexpr int kFixed = kQBytes + 2 * kPBytes;
-  // as many KV stages as fit next to Q and the two P buffers (227 KB per CTA), at most 4
-  static constexpr int kFit = (232448 - 2048 - kFixed) / kStageBytes;
+  // as many KV stages as fit next to Q (227 KB per CTA), at most 4
+  static constexpr int kFit = (232448 - 2048 - kQBytes) / kStageBytes;
   static constexpr int kStages = kFit > 4 ? 4 : kFit;
-  static constexpr int kBarOff = kFixed + kStages * kStageBytes;
+  static constexpr int kBarOff = kQBytes + kStages * kStageBytes;
   static constexpr int kBytes = kBarOff + 256 + 1024;
-  static constexpr int kTmemCols = (2 * KV + D) <= 128 ? 128 : ((2 * KV + D) <= 256 ? 256 : 512);
   static_assert(kStages >= 2, "needs two KV stages");
-  static_assert(2 * KV + D <= 512, "TMEM budget");
 };
-
-__device__ __forceinline__ void tmem_st_32x32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      :
-      : "r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-        "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]),
-        "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]),
-        "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// SW128 descriptor with explicit LBO / SBO (MN-major operands use both)
-__device__ __forceinline__ uint64_t make_sw128_desc(uint32_t smem_addr, uint32_t lbo16, uint32_t sbo16) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFF);
-  d |= static_cast<uint64_t>(lbo16 & 0x3FFF) << 16;
-  d |= static_cast<uint64_t>(sbo16 & 0x3FFF) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
-  return d;
-}
 
 // byte offset of (row, 16-byte chunk c) in a K-major SW128 operand tile stored as [c / 8][128 rows][128 B]
 __device__ __forceinline__ uint32_t a_tile_off(int row, int c) {
@@ -101,16 +62,10 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmap_k, const __grid_
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sq = smem;
-  uint8_t* sp = smem + SM::kQBytes;                    // two P buffers
-  uint8_t* skv = sp + 2 * SM::kPBytes;                 // KV ring
+  uint8_t* skv = smem + SM::kQBytes;                   // KV ring
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + SM::kBarOff);
-  uint64_t* kv_full = bars;                            // [kStages]  TMA -> MMA
-  uint64_t* kv_empty = kv_full + SM::kStages;          // [kStages]  PV commit -> producer
-  uint64_t* s_full = kv_empty + SM::kStages;           // [2]        QK^T commit -> softmax
-  uint64_t* p_full = s_full + 2;                       // [2]        softmax (128 arrivals) -> MMA
-  uint64_t* pv_done = p_full + 2;                      // [2]        PV commit -> softmax (O readable, P buffer free)
-  uint64_t* q_full = pv_done + 2;                      // [1]        Q staged (128 arrivals)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(q_full + 1);
+  uint64_t* kv_full = bars;                            // [kStages]  TMA -> MMA warpgroups
+  uint64_t* kv_empty = kv_full + SM::kStages;          // [kStages]  8 consumer warps -> producer
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int seq = blockIdx.y + p.seq_offset;
@@ -132,26 +87,16 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmap_k, const __grid_
   if (threadIdx.x == 0) {
     for (int i = 0; i < SM::kStages; ++i) {
       mbar_init(&kv_full[i], 1);
-      mbar_init(&kv_empty[i], 1);
+      mbar_init(&kv_empty[i], 8);
     }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&s_full[i], 1);
-      mbar_init(&p_full[i], kTcSoftmaxWarps * 32);
-      mbar_init(&pv_done[i], 1);
-    }
-    mbar_init(q_full, kTcSoftmaxWarps * 32);
     fence_mbar_init();
   }
-  if (warp == kTcSoftmaxWarps + 1) tmem_alloc<1>(tmem_slot, SM::kTmemCols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
-  const uint32_t tmem_o = tmem + 2 * KV;
 
-  if (warp == kTcSoftmaxWarps) {
+  if (warp < 4) {
     // ------------------------------------------------------------------ TMA producer
-    if (lane == 0) {
+    regs_dealloc<40>();
+    if (warp == 0 && lane == 0) {
       const int32_t* bt = p.block_table + static_cast<size_t>(seq) * p.max_blocks;
       const int pages_per_tile = KV / p.page_size;
       const int page_rows_bytes = p.page_size * 128;
@@ -176,194 +121,134 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tmap_k, const __grid_
         }
       }
     }
-  } else if (warp == kTcSoftmaxWarps + 1) {
-    // ------------------------------------------------------------------ MMA issuer
-    if (lane == 0) {
-      constexpr uint32_t idesc_s = make_idesc_bf16(kTcRows, KV);
-      const uint32_t nv = p.v_split_n ? 64u : static_cast<uint32_t>(D);
-      const uint32_t idesc_pv = (1u << 4) | (1u << 7) | (1u << 10) | (1u << 16) | ((nv >> 3) << 17) | ((kTcRows >> 4) << 24);
-      const uint32_t q_addr = smem_u32(sq);
-      auto issue_s = [&](int tile) {
-        const int s = tile % SM::kStages;
-        mbar_wait(&kv_full[s], (tile / SM::kStages) & 1);
-        tc_fence_after();
-        const uint32_t k_addr = smem_u32(skv + s * SM::kStageBytes);
-        const uint32_t d_tmem = tmem + (tile & 1) * KV;
-#pragma unroll
-        for (int kd = 0; kd < D / 64; ++kd) {
-          const uint64_t da = make_sw128_kmajor_desc(q_addr + kd * (kTcRows * 128));
-          const uint64_t db = make_sw128_kmajor_desc(k_addr + kd * (KV * 128));
-#pragma unroll
-          for (int kk = 0; kk < 4; ++kk) umma_bf16<1>(d_tmem, da + kk * 2, db + kk * 2, idesc_s, (kd | kk) != 0);
-        }
-        umma_commit(&s_full[tile & 1]);
-      };
-      mbar_wait(q_full, 0);
-      tc_fence_after();
-      issue_s(0);
-      for (int tile = 0; tile < n_tiles; ++tile) {
-        if (tile + 1 < n_tiles) issue_s(tile + 1);      // runs under the softmax of `tile`
-        const int b = tile & 1;
-        mbar_wait(&p_full[b], (tile >> 1) & 1);
-        tc_fence_after();
-        const int s = tile % SM::kStages;
-        const uint32_t v_addr = smem_u32(skv + s * SM::kStageBytes + SM::kTileBytes);
-        const uint32_t p_addr = smem_u32(sp + b * SM::kPBytes);
-#pragma unroll
-        for (int ks = 0; ks < KV / 64; ++ks) {
-          const uint64_t da = make_sw128_kmajor_desc(p_addr + ks * (kTcRows * 128));
-#pragma unroll
-          for (int kk = 0; kk < 4; ++kk) {
-            const int kstep = ks * 4 + kk;               // 16 keys per step
-            const uint32_t acc = (tile | kstep) != 0;
-            const uint64_t dv = make_sw128_desc(v_addr, p.v_lbo16, p.v_sbo16) + static_cast<uint64_t>(kstep) * p.v_kadv16;
-            if (p.v_split_n) {
-#pragma unroll
-              for (int nd = 0; nd < D / 64; ++nd)
-                umma_bf16<1>(tmem_o + nd * 64, da + kk * 2, dv + static_cast<uint64_t>(nd) * ((KV * 128) >> 4),
-                             idesc_pv, acc);
-            } else {
-              umma_bf16<1>(tmem_o, da + kk * 2, dv, idesc_pv, acc);
-            }
-          }
-        }
-        umma_commit(&kv_empty[s]);                       // K and V of this stage consumed
-        umma_commit(&pv_done[b]);                        // O holds tiles 0..tile; P buffer b is free
-      }
-    }
-  } else {
-    // ------------------------------------------------------------------ softmax warps: one row per thread
-    const int row = threadIdx.x;                         // 0..127 == TMEM lane
+    return;
+  }
+  // -------------------------------------------------------------------- MMA + softmax warpgroups
+  regs_alloc<232>();
+  const int ct = threadIdx.x - 128;                    // 0..255
+  const int g = ct >> 7;
+  const int wq = (ct >> 5) & 3;
+  {  // stage Q as the K-major SW128 A operand: thread ct copies row ct / 2, half (ct & 1) of the head dim
+    const int row = ct >> 1;
     const int tok = tok_base + row / p.GP;
     const int head = hbase + row % p.GP;
-    const bool row_ok = tok < q_len;
-    const uint32_t lane_base = static_cast<uint32_t>(warp * 32) << 16;
-    {  // stage Q as the K-major SW128 A operand
-      const uint4* qp = reinterpret_cast<const uint4*>(p.q + static_cast<size_t>(q_begin + (row_ok ? tok : 0)) * p.q_ts +
-                                                       static_cast<size_t>(head) * D);
+    const bool ok = tok < q_len;
+    const uint4* qp = reinterpret_cast<const uint4*>(p.q + static_cast<size_t>(q_begin + (ok ? tok : 0)) * p.q_ts +
+                                                     static_cast<size_t>(head) * D);
 #pragma unroll
-      for (int c = 0; c < D / 8; ++c) {
-        uint4 v = make_uint4(0u, 0u, 0u, 0u);
-        if (row_ok) v = ld_nc_v4(qp + c);
-        *reinterpret_cast<uint4*>(sq + a_tile_off(row, c)) = v;
-      }
-      fence_proxy_async_smem();
-      mbar_arrive(q_full);
+    for (int c0 = 0; c0 < D / 16; ++c0) {
+      const int c = (ct & 1) * (D / 16) + c0;
+      uint4 v = make_uint4(0u, 0u, 0u, 0u);
+      if (ok) v = ld_nc_v4(qp + c);
+      *reinterpret_cast<uint4*>(sq + a_tile_off(row, c)) = v;
     }
-    const int lim = ctx_len + tok;                       // last visible key of this row
-    float m_run = -INFINITY, l_run = 0.f;
-    for (int tile = 0; tile < n_tiles; ++tile) {
-      const int b = tile & 1;
-      mbar_wait(&s_full[b], (tile >> 1) & 1);
-      tc_fence_after();
-      const uint32_t t_s = tmem + lane_base + b * KV;
-      const int key0 = tile * KV;
-      const bool need_mask = key0 + KV - 1 > ctx_len + tok_base;   // CTA-uniform: a diagonal tile
-      // pass 1: row max
-      float mx = -INFINITY;
-#pragma unroll 1
-      for (int c = 0; c < KV; c += 32) {
-        uint32_t v[32];
-        tmem_ld_32x32(t_s + c, v);
-        tmem_ld_wait();
-        if (need_mask) {
-#pragma unroll
-          for (int e = 0; e < 32; ++e) mx = fmaxf(mx, (key0 + c + e <= lim) ? __uint_as_float(v[e]) : -INFINITY);
-        } else {
-#pragma unroll
-          for (int e = 0; e < 32; ++e) mx = fmaxf(mx, __uint_as_float(v[e]));
-        }
-      }
-      const float m_new = fmaxf(m_run, mx * p.scale_log2);
-      const float m_use = (m_new == -INFINITY) ? 0.f : m_new;
-      const float alpha = exp2f(m_run - m_use);
-      m_run = m_new;
-      // pass 2: P = exp2(S * scale - m), row sum, bf16 P -> smem (A operand of the PV product)
-      uint8_t* pb = sp + b * SM::kPBytes;
-      float sum = 0.f;
-#pragma unroll 1
-      for (int c = 0; c < KV; c += 32) {
-        uint32_t v[32];
-        tmem_ld_32x32(t_s + c, v);
-        tmem_ld_wait();
-        float f[32];
-#pragma unroll
-        for (int e = 0; e < 32; ++e) {
-          float x = exp2f(fmaf(__uint_as_float(v[e]), p.scale_log2, -m_use));
-          if (need_mask && key0 + c + e > lim) x = 0.f;
-          f[e] = x;
-          sum += x;
-        }
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          uint4 w;
-          w.x = pack_bf16(f[g * 8 + 0], f[g * 8 + 1]);
-          w.y = pack_bf16(f[g * 8 + 2], f[g * 8 + 3]);
-          w.z = pack_bf16(f[g * 8 + 4], f[g * 8 + 5]);
-          w.w = pack_bf16(f[g * 8 + 6], f[g * 8 + 7]);
-          *reinterpret_cast<uint4*>(pb + a_tile_off(row, (c >> 3) + g)) = w;
-        }
-      }
-      l_run = l_run * alpha + sum;
-      fence_proxy_async_smem();                          // P visible to the tensor core (async proxy)
-      tc_fence_before();                                 // the S reads above are ordered before the arrive
-      if (tile > 0) {
-        // O is rescaled in TMEM only if some row of this warp moved its max; PV(tile-1) must have landed first
-        mbar_wait(&pv_done[b ^ 1], ((tile - 1) >> 1) & 1);
-        tc_fence_after();
-        if (__any_sync(0xffffffffu, alpha != 1.f)) {
-          const uint32_t t_o = tmem_o + lane_base;
-#pragma unroll 1
-          for (int c = 0; c < D; c += 32) {
-            uint32_t v[32];
-            tmem_ld_32x32(t_o + c, v);
-            tmem_ld_wait();
-#pragma unroll
-            for (int e = 0; e < 32; ++e) v[e] = __float_as_uint(__uint_as_float(v[e]) * alpha);
-            tmem_st_32x32(t_o + c, v);
-          }
-          tmem_st_wait();
-        }
-        tc_fence_before();
-      }
-      mbar_arrive(&p_full[b]);
-    }
-    // ---- epilogue: O / l -> bf16 -> global
-    const int lt = n_tiles - 1;
-    mbar_wait(&pv_done[lt & 1], (lt >> 1) & 1);
-    tc_fence_after();
-    const float inv = l_run > 0.f ? 1.f / l_run : 0.f;
-    __nv_bfloat16* op = p.out + (static_cast<size_t>(q_begin + tok) * p.Hq + head) * D;
-    const uint32_t t_o = tmem_o + lane_base;
-#pragma unroll 1
-    for (int c = 0; c < D; c += 32) {
-      uint32_t v[32];
-      tmem_ld_32x32(t_o + c, v);
-      tmem_ld_wait();
-      if (row_ok) {
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          uint4 w;
-          w.x = pack_bf16(__uint_as_float(v[g * 8 + 0]) * inv, __uint_as_float(v[g * 8 + 1]) * inv);
-          w.y = pack_bf16(__uint_as_float(v[g * 8 + 2]) * inv, __uint_as_float(v[g * 8 + 3]) * inv);
-          w.z = pack_bf16(__uint_as_float(v[g * 8 + 4]) * inv, __uint_as_float(v[g * 8 + 5]) * inv);
-          w.w = pack_bf16(__uint_as_float(v[g * 8 + 6]) * inv, __uint_as_float(v[g * 8 + 7]) * inv);
-          *reinterpret_cast<uint4*>(op + c + g * 8) = w;
-        }
-      }
-    }
-    tc_fence_before();
+    fence_proxy_async_smem();                          // Q visible to the tensor core (async proxy)
+    asm volatile("bar.sync 1, 256;" ::: "memory");
   }
-  __syncthreads();
-  if (warp == kTcSoftmaxWarps + 1) {
-    __syncwarp();
-    tc_fence_after();
-    tmem_dealloc<1>(tmem, SM::kTmemCols);
+  // fragment rows of this thread: r[h] = 64 g + 16 wq + lane / 4 + 8 h; columns 8 j + 2 (lane % 4) + {0, 1}
+  int tok[2], head[2], lim[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int row = 64 * g + 16 * wq + (lane >> 2) + 8 * h;
+    tok[h] = tok_base + row / p.GP;
+    head[h] = hbase + row % p.GP;
+    lim[h] = ctx_len + tok[h];                         // last visible key of this row
+  }
+  const int cq = 2 * (lane & 3);
+  const uint32_t q_addr = smem_u32(sq) + g * (64 * 128);
+  float o[D / 2];
+#pragma unroll
+  for (int i = 0; i < D / 2; ++i) o[i] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+  for (int tile = 0; tile < n_tiles; ++tile) {
+    const int s = tile % SM::kStages;
+    mbar_wait(&kv_full[s], (tile / SM::kStages) & 1);
+    const uint32_t k_addr = smem_u32(skv + s * SM::kStageBytes);
+    const uint32_t v_addr = k_addr + SM::kTileBytes;
+    float sc[KV / 2];
+    wgmma_fence();
+#pragma unroll
+    for (int kd = 0; kd < D / 64; ++kd) {
+      const uint64_t da = make_sw128_kmajor_desc(q_addr + kd * (kTcRows * 128));
+      const uint64_t db = make_sw128_kmajor_desc(k_addr + kd * (KV * 128));
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) wgmma_bf16_ss<KV>(sc, da + kk * 2, db + kk * 2, (kd | kk) != 0);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(sc);
+
+    const int key0 = tile * KV;
+    const bool need_mask = key0 + KV - 1 > ctx_len + tok_base;   // CTA-uniform: a diagonal tile
+    if (need_mask) {
+#pragma unroll
+      for (int j = 0; j < KV / 8; ++j)
+#pragma unroll
+        for (int e = 0; e < 4; ++e)
+          if (key0 + 8 * j + cq + (e & 1) > lim[e >> 1]) sc[4 * j + e] = -INFINITY;
+    }
+    float alpha[2], m_use[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float mx = -INFINITY;
+#pragma unroll
+      for (int j = 0; j < KV / 8; ++j) mx = fmaxf(mx, fmaxf(sc[4 * j + 2 * h], sc[4 * j + 2 * h + 1]));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float m_new = fmaxf(m_run[h], mx * p.scale_log2);
+      m_use[h] = (m_new == -INFINITY) ? 0.f : m_new;
+      alpha[h] = exp2f(m_run[h] - m_use[h]);
+      m_run[h] = m_new;
+    }
+    // P = exp2(S * scale - m) as bf16 A fragments (k16 chunk t: keys 16 t .. 16 t + 15), per-thread row sums
+    uint32_t pa[KV / 16][4];
+    float sum[2] = {0.f, 0.f};
+#pragma unroll
+    for (int j = 0; j < KV / 8; ++j) {
+      float x[4];
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        x[e] = exp2f(fmaf(sc[4 * j + e], p.scale_log2, -m_use[e >> 1]));
+        sum[e >> 1] += x[e];
+      }
+      pa[j >> 1][(j & 1) * 2] = pack_bf16(x[0], x[1]);
+      pa[j >> 1][(j & 1) * 2 + 1] = pack_bf16(x[2], x[3]);
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) l_run[h] = l_run[h] * alpha[h] + sum[h];
+#pragma unroll
+    for (int j = 0; j < D / 8; ++j) {
+      o[4 * j] *= alpha[0]; o[4 * j + 1] *= alpha[0];
+      o[4 * j + 2] *= alpha[1]; o[4 * j + 3] *= alpha[1];
+    }
+    wgmma_fence();
+#pragma unroll
+    for (int t = 0; t < KV / 16; ++t) {
+      const uint64_t dv = make_sw128_desc(v_addr + t * 2048, (KV * 128) >> 4, 1024 >> 4);
+      wgmma_bf16_rs_tb<D>(o, pa[t], dv, 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(o);
+    if (lane == 0) mbar_arrive(&kv_empty[s]);          // K and V of this stage consumed
+  }
+  // ---- epilogue: O / l -> bf16 -> global
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float l = l_run[h];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    const float inv = l > 0.f ? 1.f / l : 0.f;
+    if (tok[h] >= q_len) continue;
+    __nv_bfloat16* op = p.out + (static_cast<size_t>(q_begin + tok[h]) * p.Hq + head[h]) * D;
+#pragma unroll
+    for (int j = 0; j < D / 8; ++j)
+      *reinterpret_cast<uint32_t*>(op + 8 * j + cq) = pack_bf16(o[4 * j + 2 * h] * inv, o[4 * j + 2 * h + 1] * inv);
   }
 }
 
 // tensor map over the paged cache with ONE 64-wide slab per box ([page_size][64]), so that a KV tile can be
-// assembled slab-major ([D/64][KV][64]) — the layout both UMMA operand forms need
+// assembled slab-major ([D/64][KV][64]) — the layout both wgmma operand forms need
 static int get_kv_slab_tmap(const void* base, int64_t num_pages, int Hkv, int D, int page_size, CUtensorMap* out) {
   static std::unordered_map<TmapKey, CUtensorMap, TmapKeyHash> cache;
   static std::mutex mu;
@@ -439,17 +324,6 @@ GLLM_EXPORT int gllm_attn_prefill_tc(const void* q, int64_t q_ts, void* out, con
     if (p.G % d == 0 && kTcRows % d == 0) { p.GP = d; break; }
   p.page_size = page_size; p.seq_offset = seq_offset;
   p.scale_log2 = scale * 1.4426950408889634f;
-  // MN-major V operand (see the header comment); overridable for bring-up
-  p.v_lbo16 = static_cast<uint32_t>(kv_tile * 128) >> 4;
-  p.v_sbo16 = 1024 >> 4;
-  p.v_kadv16 = 2048 >> 4;
-  p.v_split_n = 0;
-  if (const char* e = getenv("GLLM_ATTN_TC_V")) {
-    unsigned a, b, c, d2;
-    if (sscanf(e, "%u,%u,%u,%u", &a, &b, &c, &d2) == 4) {
-      p.v_lbo16 = a; p.v_sbo16 = b; p.v_kadv16 = c; p.v_split_n = d2;
-    }
-  }
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   if (D == 128) {
     return kv_tile == 128 ? launch_prefill_tc<128, 128>(tk, tv, p, num_seqs, max_q_len, st)

@@ -4,7 +4,7 @@
 //
 //   dispatch   every (token, top-k choice) of this rank's shard claims a row in the EXPERT OWNER's receive
 //              pool with one remote atomic and stores the token row + (local expert, source) there (P2P st)
-//   experts    the owner runs align -> grouped tcgen05 GEMM1 (SiLU gate) -> grouped GEMM2 over the pool;
+//   experts    the owner runs align -> grouped wgmma GEMM1 (SiLU gate) -> grouped GEMM2 over the pool;
 //              GEMM2's epilogue stores every output row straight into the TOKEN OWNER's combine buffer
 //              through a per-row destination table (gemm_bf16.cu `row_dest`) — the return all-to-all is the
 //              GEMM epilogue, there is no separate send

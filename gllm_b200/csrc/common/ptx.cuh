@@ -1,5 +1,5 @@
-// Thin inline-PTX wrappers for the Blackwell (sm_100a) programming model:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld),
+// Thin inline-PTX wrappers for the Hopper (sm_90a) programming model:
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma (descriptors / fences / commit groups),
 // and system-scope flag synchronisation for peer memory.
 //
 // Everything here is written against the PTX ISA directly; there is no CUTLASS
@@ -10,6 +10,8 @@
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include "wgmma.cuh"
 
 namespace b200 {
 
@@ -116,123 +118,42 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const void* tmap, ui
 }
 
 // ----------------------------------------------------------------------------
-// tcgen05: TMEM allocation, MMA, commit, load
+// wgmma: warpgroup MMA with shared-memory descriptors, fences, register budgets
 // ----------------------------------------------------------------------------
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-
-// Must be executed by one full warp. Result (TMEM base address) lands in *dst_smem.
-template <int kCtaGroup = 1>
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  static_assert(kCtaGroup == 1, "every kernel in this library issues single-CTA tcgen05 (cta_group::1)");
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-
-template <int kCtaGroup = 1>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  static_assert(kCtaGroup == 1, "single-CTA tcgen05 only");
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-
-// Shared-memory matrix descriptor for a K-major operand tile stored with the
-// 128-byte swizzle (one swizzle atom == 8 rows x 128 B). `row_bytes` must be 128.
-// SBO = stride between 8-row groups = 1024 B. LBO is unused for swizzled K-major.
-__device__ __forceinline__ uint64_t make_sw128_kmajor_desc(uint32_t smem_addr) {
+// Shared-memory matrix descriptor (sm_90) for an operand tile stored with the 128-byte swizzle
+// (one swizzle atom == 8 rows x 128 B). K-major: SBO = stride between 8-row groups (1024 B), LBO unused.
+// MN-major: LBO = stride between 64-element column chunks, SBO = stride between 8-row K groups.
+__device__ __forceinline__ uint64_t make_sw128_desc(uint32_t smem_addr, uint32_t lbo16, uint32_t sbo16) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFF);  // start address
-  d |= static_cast<uint64_t>(0) << 16;                    // LBO (ignored)
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;            // SBO
-  d |= static_cast<uint64_t>(1) << 46;                    // descriptor version (sm_100)
-  d |= static_cast<uint64_t>(2) << 61;                    // SWIZZLE_128B
+  d |= static_cast<uint64_t>(lbo16 & 0x3FFF) << 16;       // leading-dimension byte offset
+  d |= static_cast<uint64_t>(sbo16 & 0x3FFF) << 32;       // stride-dimension byte offset
+  d |= static_cast<uint64_t>(1) << 62;                    // SWIZZLE_128B
   return d;
 }
 
-// Instruction descriptor for kind::f16 (bf16 x bf16 -> fp32), both operands K-major.
-__host__ __device__ constexpr uint32_t make_idesc_bf16(uint32_t m, uint32_t n) {
-  return (1u << 4)            // D format: f32
-         | (1u << 7)          // A format: bf16
-         | (1u << 10)         // B format: bf16
-         | (0u << 15)         // A K-major
-         | (0u << 16)         // B K-major
-         | ((n >> 3) << 17)   // N / 8
-         | ((m >> 4) << 24);  // M / 16
+__device__ __forceinline__ uint64_t make_sw128_kmajor_desc(uint32_t smem_addr) {
+  return make_sw128_desc(smem_addr, 1, 1024 >> 4);
 }
 
-// kind::f8f6f4 with e4m3 operands, fp32 accumulate.
-__host__ __device__ constexpr uint32_t make_idesc_e4m3(uint32_t m, uint32_t n) {
-  return (1u << 4) | (0u << 7) | (0u << 10) | ((n >> 3) << 17) | ((m >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+// keep the accumulator registers live across wgmma_wait (the compiler must not move reads above it)
+template <int N>
+__device__ __forceinline__ void reg_fence(float (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-template <int kCtaGroup = 1>
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                          uint32_t idesc, uint32_t accumulate) {
-  static_assert(kCtaGroup == 1, "single-CTA tcgen05 only");
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-__device__ __forceinline__ void umma_f8(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                        uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f8f6f4 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-// Make the mbarrier track completion of all prior tcgen05 async ops of this thread.
-// (implicitly performs tcgen05.fence::before_thread_sync)
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   smem_u32(bar))
-               : "memory");
-}
-
-// TMEM -> registers: 32 lanes x 32 columns of fp32 (each thread: its lane, 32 columns).
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
+// warpgroup register budgets: producer warpgroups give registers to the MMA warpgroups
+template <int R>
+__device__ __forceinline__ void regs_dealloc() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void regs_alloc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 
 // ----------------------------------------------------------------------------
 // global memory helpers (vector, cache-hinted, system-scope flags for NVLink peers)

@@ -1,4 +1,4 @@
-// RMSNorm (+ fused residual add) and SiLU-gate for sm_100a.
+// RMSNorm (+ fused residual add) and SiLU-gate for sm_90a.
 //
 // Memory-bound row kernels: 16-byte vector loads/stores, the row stays in registers between
 // the reduction and the scale pass, one CTA per token row. They replace the reference's

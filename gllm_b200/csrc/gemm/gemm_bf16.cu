@@ -1,13 +1,11 @@
-// Persistent, warp-specialised bf16 GEMM for sm_100a:
+// Persistent, warp-specialised bf16 GEMM for sm_90a:
 //
 //     C[M, N] = A[M, K] · W[N, K]^T  (+ bias)           (nn.Linear layout, both K-major)
 //
-//   * operands staged by TMA (128-byte swizzle) through an mbarrier ring,
-//   * tcgen05.mma (kind::f16, 128 x BN x 16) issued by one elected thread,
-//   * fp32 accumulators double-buffered in TMEM so the epilogue of tile i overlaps the
-//     main loop of tile i+1,
-//   * four epilogue warps drain TMEM with tcgen05.ld and apply the fused epilogue
-//     (bias, SiLU-gate for the merged gate/up projection),
+//   * operands staged by TMA (128-byte swizzle) through an mbarrier ring filled by one producer warp,
+//   * two consumer warpgroups, each multiplying 64 rows of the 128 x BN tile with wgmma.mma_async
+//     (m64nBNk16, both operands from shared memory, fp32 accumulators in registers),
+//   * the consumers apply the fused epilogue (bias, SiLU-gate for the merged gate/up projection),
 //   * optional fused collectives over NVLink peer memory (SURVEY §2.4 X1/X2):
 //       - all-gather ⊕ GEMM: the TMA producer gates each M tile on per-row-block
 //         "ready" flags that peer ranks set after pushing their activation shard,
@@ -24,8 +22,9 @@ namespace b200 {
 
 static constexpr int kBlockM = 128;
 static constexpr int kBlockK = 64;  // 64 bf16 = 128 B = one swizzle atom row
-static constexpr int kUmmaK = 16;
-static constexpr int kNumThreads = 192;  // warp0: TMA, warp1: MMA, warps2-5: epilogue
+static constexpr int kMmaK = 16;
+static constexpr int kNumThreads = 384;  // warpgroup 0: TMA producer, warpgroups 1-2: MMA + epilogue
+static constexpr int kConsumers = 256;
 static constexpr int kMaxPeers = 8;
 
 enum Epilogue : int { kEpiStore = 0, kEpiSiluMul = 1 };
@@ -72,13 +71,12 @@ struct GemmCfg {
   static constexpr int kABytes = kBlockM * kBlockK * 2;
   static constexpr int kBBytes = BN * kBlockK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  // epilogue staging: 4 warps x 32 rows x 64 output columns (bf16) + 4 x 32 destination row pointers
-  static constexpr int kEpiBytes = 4 * 32 * 128 + 4 * 32 * 8 + 16;
-  static constexpr int kSmemBudget = 220 * 1024 - kEpiBytes;
+  // epilogue staging: 8 warps x 16 rows x 64 output columns (bf16) + 8 x 16 destination row pointers
+  static constexpr int kEpiBytes = 8 * 16 * 128 + 8 * 16 * 8;
+  static constexpr int kSmemBudget = 224 * 1024 - kEpiBytes;
   static constexpr int kStagesRaw = kSmemBudget / kStageBytes;
   static constexpr int kStages = kStagesRaw > 8 ? 8 : kStagesRaw;
-  static constexpr int kTmemCols = (2 * BN <= 32) ? 32 : (2 * BN <= 64) ? 64 : (2 * BN <= 128) ? 128 : (2 * BN <= 256) ? 256 : 512;
-  // barriers: full[S], empty[S], tmem_full[2], tmem_empty[2] + tmem ptr
+  // barriers: full[S], empty[S]
   static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align*/ + 256 + kEpiBytes;
 };
 
@@ -88,14 +86,12 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
                  const GemmParams p) {
   using Cfg = GemmCfg<BN>;
   constexpr int S = Cfg::kStages;
+  constexpr int NACC = BN / 2;  // fp32 accumulators per consumer thread (64 x BN per warpgroup)
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + S * Cfg::kStageBytes);
   uint64_t* empty_bar = full_bar + S;
-  uint64_t* tmem_full = empty_bar + S;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(tmem_empty + 2);
   uint8_t* epi_smem = smem + S * Cfg::kStageBytes + 256;
 
   const int warp = threadIdx.x >> 5;
@@ -124,25 +120,16 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     tma_prefetch_desc(&tmap_b);
     for (int i = 0; i < S; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], 4);
+      mbar_init(&empty_bar[i], kConsumers / 32);
     }
     fence_mbar_init();
   }
-  if (warp == 1) {
-    tmem_alloc<1>(tmem_ptr_smem, Cfg::kTmemCols);
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    if (lane == 0) {
+  if (warp < 4) {
+    // ===================== TMA producer (one thread) =====================
+    regs_dealloc<40>();
+    if (warp == 0 && lane == 0) {
       uint32_t it = 0;
       // weights (B) do not depend on the previous kernel: put the first stages' B tiles in flight, then wait
       uint32_t pre = 0;
@@ -198,170 +185,147 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc_bf16(kBlockM, BN);
-      uint32_t it = 0;
-      uint32_t tcount = 0;
-      for (int unit = blockIdx.x; unit < num_units; unit += gridDim.x, ++tcount) {
-        const int kb0 = (unit % split) * kpb;
-        const int kb1 = min(num_kb, kb0 + kpb);
-        const uint32_t buf = tcount & 1;
-        const uint32_t aph = (tcount >> 1) & 1;
-        mbar_wait(&tmem_empty[buf], aph ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + buf * BN;
-        for (int kb = kb0; kb < kb1; ++kb, ++it) {
-          const int s = it % S;
-          const uint32_t ph = (it / S) & 1;
-          mbar_wait(&full_bar[s], ph);
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(smem + s * Cfg::kStageBytes);
-          const uint32_t b_addr = a_addr + Cfg::kABytes;
-          const uint64_t da = make_sw128_kmajor_desc(a_addr);
-          const uint64_t db = make_sw128_kmajor_desc(b_addr);
-#pragma unroll
-          for (int k = 0; k < kBlockK / kUmmaK; ++k) {
-            // advance 32 B (16 bf16) along K inside the swizzle atom: +2 in 16-byte units
-            umma_bf16<1>(d_tmem, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), idesc,
-                         (kb > kb0 || k > 0) ? 1u : 0u);
-          }
-          umma_commit(&empty_bar[s]);
-        }
-        umma_commit(&tmem_full[buf]);
-      }
-    }
   } else {
-    // ===================== epilogue warps =====================
+    // ===================== MMA + epilogue warpgroups =====================
+    regs_alloc<232>();
     if (!grouped) griddep_wait();
-    const int q = warp & 3;  // TMEM lane quarter this warp may access
-    uint32_t tcount = 0;
-    for (int unit = blockIdx.x; unit < num_units; unit += gridDim.x, ++tcount) {
+    const int ct = threadIdx.x - 128;   // consumer thread 0..255
+    const int g = ct >> 7;              // warpgroup: rows [64 g, 64 g + 64) of the tile
+    const int wq = (ct >> 5) & 3;       // warp inside the warpgroup: 16 rows each
+    const int cw = ct >> 5;             // consumer warp 0..7
+    // accumulator fragment: acc[4 j + {0,1}] = (row r0, cols 8 j + 2 (lane % 4) + {0,1}), acc[4 j + {2,3}] = row r0 + 8
+    const int cq = 2 * (lane & 3);
+    uint32_t it = 0;
+    for (int unit = blockIdx.x; unit < num_units; unit += gridDim.x) {
       const int tile = unit / split;
+      const int kb0 = (unit - tile * split) * kpb;
+      const int kb1 = min(num_kb, kb0 + kpb);
       const int m0 = (((tile % num_m) + p.m_rot) % num_m) * kBlockM;
       const int n0 = (tile / num_m) * BN;
-      const uint32_t buf = tcount & 1;
-      const uint32_t aph = (tcount >> 1) & 1;
-      mbar_wait(&tmem_full[buf], aph);
-      tc_fence_after();
-      int row = m0 + q * 32 + lane;
-      bool row_in = row < p.M;
-      int64_t c_off = 0;
-      if (p.batch > 0) {   // tile -> (batch entry, row inside it)
-        const int mt = m0 / kBlockM, bidx = mt / tpb;
-        row = (mt - bidx * tpb) * kBlockM + q * 32 + lane;
-        row_in = row < p.rows_per_batch;
-        c_off = static_cast<int64_t>(bidx) * p.c_batch_stride;
-      }
-      const uint32_t t_row = tmem_base + buf * BN + (static_cast<uint32_t>(q * 32) << 16);
 
-      // destination row pointer (local C, or the owner rank's staging buffer for RS)
-      __nv_bfloat16* crow = nullptr;
-      int out_n0 = (EPI == kEpiSiluMul) ? n0 / 2 : n0;
-      const int out_N = (EPI == kEpiSiluMul) ? p.N / 2 : p.N;
-      bool row_ok = row_in;
-      if (row_in && p.row_dest != nullptr) {
-        crow = reinterpret_cast<__nv_bfloat16*>(p.row_dest[row]);
-        row_ok = crow != nullptr;
-      } else if (row_ok) {
-        if (p.rs_world > 0) {
-          const int owner = p.rs_bcast ? 0 : row / p.rows_per_rank;
-          const int r_local = row - owner * p.rows_per_rank;
-          crow = p.peer_out[owner] +
-                 (static_cast<size_t>(p.rs_rank) * p.rows_per_rank + r_local) * p.ldc;
-        } else {
-          crow = p.C + static_cast<size_t>(row) * p.ldc + c_off;
-        }
-      }
-
-      constexpr int OUT_W_ = (EPI == kEpiSiluMul) ? BN / 2 : BN;
-      // thread-private workspace layout: [unit][warp q][32-col chunk][j][lane] float4 — the reader of a value
-      // is the thread (q, lane) that wrote it, so every access is a fully coalesced 512-byte warp transaction
-      auto ws_ptr = [&](int u, int chunk, int j) {
-        return reinterpret_cast<float4*>(p.ws) +
-               ((((static_cast<size_t>(u) * 4 + q) * (BN / 32) + chunk) * 8 + j) * 32 + lane);
-      };
-      if (split > 1) {
-#pragma unroll 1
-        for (int c = 0; c < BN; c += 32) {
-          uint32_t v[32];
-          tmem_ld_32x32(t_row + c, v);
-          tmem_ld_wait();
+      float acc[NACC];
 #pragma unroll
-          for (int j = 0; j < 8; ++j)
-            *ws_ptr(unit, c / 32, j) = make_float4(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1]),
-                                                   __uint_as_float(v[4 * j + 2]), __uint_as_float(v[4 * j + 3]));
+      for (int i = 0; i < NACC; ++i) acc[i] = 0.f;
+      // one wgmma group in flight: stage kb is released once the group of kb + 1 has been issued and kb's retired
+      int prev_s = -1;
+      for (int kb = kb0; kb < kb1; ++kb, ++it) {
+        const int s = it % S;
+        mbar_wait(&full_bar[s], (it / S) & 1);
+        const uint32_t a_addr = smem_u32(smem + s * Cfg::kStageBytes) + g * (64 * 128);
+        const uint32_t b_addr = smem_u32(smem + s * Cfg::kStageBytes + Cfg::kABytes);
+        const uint64_t da = make_sw128_kmajor_desc(a_addr);
+        const uint64_t db = make_sw128_kmajor_desc(b_addr);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kBlockK / kMmaK; ++k) {
+          // advance 32 B (16 bf16) along K inside the swizzle atom: +2 in 16-byte units
+          wgmma_bf16_ss<BN>(acc, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (kb > kb0 || k > 0) ? 1u : 0u);
         }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tmem_empty[buf]);
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev_s >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_s]);
+        prev_s = s;
+      }
+      wgmma_wait<0>();
+      reg_fence(acc);
+      if (prev_s >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_s]);
+
+      int64_t c_off = 0;
+      if (p.batch > 0) c_off = static_cast<int64_t>((m0 / kBlockM) / tpb) * p.c_batch_stride;
+      const int out_N = (EPI == kEpiSiluMul) ? p.N / 2 : p.N;
+      const int out_n0 = (EPI == kEpiSiluMul) ? n0 / 2 : n0;
+      constexpr int OUT_W = (EPI == kEpiSiluMul) ? BN / 2 : BN;   // output columns of this tile
+
+      if (split > 1) {
+        // thread-private workspace layout: [unit][j][consumer thread] float4 — the reader of a value is the thread
+        // that wrote it, so every access is a fully coalesced 512-byte warp transaction
+        auto ws_ptr = [&](int u, int j) {
+          return reinterpret_cast<float4*>(p.ws) + ((static_cast<size_t>(u) * (BN / 8) + j) * kConsumers + ct);
+        };
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j)
+          *ws_ptr(unit, j) = make_float4(acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3]);
         // every k-slice CTA of this tile reduces and stores its own 1/split column share (reduce-scatter
         // through L2): wait until all partners have published their partials. The partners are co-resident
         // (persistent grid, one CTA per SM, grid % split == 0 keeps a tile's slices in the same round).
         __threadfence();
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        if (warp == 2 && lane == 0) {
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+        if (ct == 0) {
           atomicAdd(p.tile_cnt + 2 * tile, 1u);
           SpinGuard guard;
           while (ld_acquire_gpu(p.tile_cnt + 2 * tile) < static_cast<uint32_t>(split)) guard.poll();
         }
-        asm volatile("bar.sync 1, 128;" ::: "memory");
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+        const int ks = unit - tile * split;
+        const int share = OUT_W / split;
+        const int c_lo = ks * share, c_hi = c_lo + share;
+        // accumulators of this unit's column share: the slice-ordered sum of the partials
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          const int oc = (EPI == kEpiSiluMul && j * 8 >= BN / 2) ? j * 8 - BN / 2 : j * 8;
+          if (oc < c_lo || oc >= c_hi) continue;
+          float4 a4 = make_float4(0.f, 0.f, 0.f, 0.f);
+          for (int sidx = 0; sidx < split; ++sidx) {
+            const float4 x = __ldcg(ws_ptr(tile * split + sidx, j));
+            a4.x += x.x; a4.y += x.y; a4.z += x.z; a4.w += x.w;
+          }
+          acc[4 * j] = a4.x; acc[4 * j + 1] = a4.y; acc[4 * j + 2] = a4.z; acc[4 * j + 3] = a4.w;
+        }
       }
       const int ks = unit - tile * split;
-      // output-column share of this unit (whole tile when split == 1)
-      const int share = OUT_W_ / split;
+      const int share = OUT_W / split;
       const int c_lo = ks * share, c_hi = c_lo + share;
-      // 32 (or 16) fp32 accumulator columns of this thread's row: from TMEM, or the slice-ordered sum of partials
-      auto load_acc = [&](int c, auto& v) {
-        constexpr int NC = sizeof(v) / sizeof(uint32_t);
-        if (split == 1) {
-          if constexpr (NC == 32) tmem_ld_32x32(t_row + c, v); else tmem_ld_32x16(t_row + c, v);
-          tmem_ld_wait();
-        } else {
-          float a[NC];
-#pragma unroll
-          for (int e = 0; e < NC; ++e) a[e] = 0.f;
-          for (int sidx = 0; sidx < split; ++sidx) {
-#pragma unroll
-            for (int j = 0; j < NC / 4; ++j) {
-              const float4 x = __ldcg(ws_ptr(tile * split + sidx, c / 32, (c % 32) / 4 + j));
-              a[4 * j] += x.x; a[4 * j + 1] += x.y; a[4 * j + 2] += x.z; a[4 * j + 3] += x.w;
-            }
-          }
-#pragma unroll
-          for (int e = 0; e < NC; ++e) v[e] = __float_as_uint(a[e]);
+
+      // destination row pointers (local C, or the owner rank's staging buffer for RS) of this warp's 16 rows
+      unsigned long long* rowptr = reinterpret_cast<unsigned long long*>(epi_smem + 8 * 16 * 128) + cw * 16;
+      if (lane < 16) {
+        const int h = lane >> 3;
+        const int rl = lane & 7;
+        // row of (lane / 4 == rl) is owned by lanes 4 rl .. 4 rl + 3; recompute it here for lane < 16
+        int row = m0 + 64 * g + 16 * wq + rl + 8 * h;
+        bool ok = row < p.M;
+        if (p.batch > 0) {
+          const int mt = m0 / kBlockM, bidx = mt / tpb;
+          row = (mt - bidx * tpb) * kBlockM + 64 * g + 16 * wq + rl + 8 * h;
+          ok = row < p.rows_per_batch;
         }
-      };
+        __nv_bfloat16* crow = nullptr;
+        if (ok && p.row_dest != nullptr) {
+          crow = reinterpret_cast<__nv_bfloat16*>(p.row_dest[row]);
+          ok = crow != nullptr;
+        } else if (ok) {
+          if (p.rs_world > 0) {
+            const int owner = p.rs_bcast ? 0 : row / p.rows_per_rank;
+            const int r_local = row - owner * p.rows_per_rank;
+            crow = p.peer_out[owner] + (static_cast<size_t>(p.rs_rank) * p.rows_per_rank + r_local) * p.ldc;
+          } else {
+            crow = p.C + static_cast<size_t>(row) * p.ldc + c_off;
+          }
+        }
+        rowptr[rl + 8 * h] = ok ? reinterpret_cast<unsigned long long>(crow) : 0ull;
+      }
 
       // Output tiles go through a per-warp swizzled smem transpose so that every global (or peer / NVLink)
-      // store instruction writes full 128-byte row segments instead of 32 scattered 16-byte pieces.
-      constexpr int OUT_W = (EPI == kEpiSiluMul) ? BN / 2 : BN;   // output columns of this tile
+      // store instruction writes full row segments instead of scattered 4-byte pieces.
       constexpr int W = OUT_W < 64 ? OUT_W : 64;                  // columns per staged chunk
       constexpr int LPR = W / 8;                                  // lanes (16 B each) per staged row
       constexpr int RPI = 32 / LPR;                               // rows per store instruction
-      uint8_t* stg = epi_smem + (warp - 2) * 4096;
-      unsigned long long* rowptr = reinterpret_cast<unsigned long long*>(epi_smem + 16384) + (warp - 2) * 32;
-      rowptr[lane] = row_ok ? reinterpret_cast<unsigned long long>(crow) : 0ull;
-      __syncwarp();
-      auto stage_put = [&](int ch, const float* f) {  // 8 consecutive output columns of this lane's row
-        uint4 o;
-        o.x = pack_bf16(f[0], f[1]);
-        o.y = pack_bf16(f[2], f[3]);
-        o.z = pack_bf16(f[4], f[5]);
-        o.w = pack_bf16(f[6], f[7]);
-        *reinterpret_cast<uint4*>(stg + lane * (W * 2) + ((ch ^ (lane & (LPR - 1) & 7)) * 16)) = o;
+      uint8_t* stg = epi_smem + cw * 2048;
+      auto stage_put = [&](int jc, int h, float f0, float f1) {   // 2 output columns of row (lane / 4 + 8 h)
+        const int r = (lane >> 2) + 8 * h;
+        *reinterpret_cast<uint32_t*>(stg + r * (W * 2) + ((jc ^ (r & (LPR - 1) & 7)) * 16) + cq * 2) =
+            pack_bf16(f0, f1);
       };
-      auto stage_flush = [&](int col0, int col_end) {  // col0: first output column of the staged chunk
+      auto stage_flush = [&](int col0, int col_lo, int col_hi) {  // col0: first output column of the staged chunk
         __syncwarp();
 #pragma unroll
-        for (int it = 0; it < 32 / RPI; ++it) {
-          const int r = it * RPI + lane / LPR;
+        for (int i2 = 0; i2 < 16 / RPI; ++i2) {
+          const int r = i2 * RPI + lane / LPR;
           const int ch = lane % LPR;
           const uint4 o = *reinterpret_cast<const uint4*>(stg + r * (W * 2) + ((ch ^ (r & (LPR - 1) & 7)) * 16));
           __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(rowptr[r]);
           const int col = col0 + ch * 8;
-          if (dst != nullptr && col < out_N && col < col_end) {
+          if (dst != nullptr && col < out_N && col >= col_lo && col < col_hi) {
             if (p.rs_bcast) {
               const ptrdiff_t delta = (dst - p.peer_out[0]) + col;
               for (int pr = 0; pr < p.rs_world; ++pr) st_v4(p.peer_out[pr] + delta, o);
@@ -373,68 +337,43 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
         __syncwarp();
       };
 
-      if constexpr (EPI == kEpiStore) {
-#pragma unroll 1
-        for (int c = c_lo; c < c_hi; c += W) {
+      __syncwarp();
 #pragma unroll
-          for (int h = 0; h < W; h += 32) {
-            if (c + h >= c_hi) break;
-            uint32_t v[32];
-            load_acc(c + h, v);
+      for (int cc = 0; cc < OUT_W; cc += W) {
+        if (cc + W <= c_lo || cc >= c_hi) continue;
 #pragma unroll
-            for (int j = 0; j < 32; j += 8) {
-              const int col = n0 + c + h + j;
-              float f[8];
-#pragma unroll
-              for (int e = 0; e < 8; ++e) f[e] = __uint_as_float(v[j + e]);
-              if (p.bias != nullptr && col < out_N) {
-                uint4 bv = *reinterpret_cast<const uint4*>(p.bias + col);
-                float2 b0 = unpack_bf16(bv.x), b1 = unpack_bf16(bv.y), b2 = unpack_bf16(bv.z),
-                       b3 = unpack_bf16(bv.w);
-                f[0] += b0.x; f[1] += b0.y; f[2] += b1.x; f[3] += b1.y;
-                f[4] += b2.x; f[5] += b2.y; f[6] += b3.x; f[7] += b3.y;
-              }
-              stage_put((h + j) / 8, f);
+        for (int jj = 0; jj < W / 8; ++jj) {
+          const int j = cc / 8 + jj;             // output column group
+          const int col = out_n0 + 8 * j + cq;
+          if constexpr (EPI == kEpiStore) {
+            float b0 = 0.f, b1 = 0.f;
+            if (p.bias != nullptr && col < out_N) {
+              const float2 bv = unpack_bf16(*reinterpret_cast<const uint32_t*>(p.bias + col));
+              b0 = bv.x; b1 = bv.y;
             }
-          }
-          stage_flush(n0 + c, n0 + c_hi);
-        }
-      } else {
-        // SiLU-gate: tile columns [0, BN/2) hold gate, [BN/2, BN) hold up for the same
-        // BN/2 output features (weights are interleaved per tile at load time).
-        constexpr int H = BN / 2;
-#pragma unroll 1
-        for (int c = c_lo; c < c_hi; c += W) {
+            stage_put(jj, 0, acc[4 * j] + b0, acc[4 * j + 1] + b1);
+            stage_put(jj, 1, acc[4 * j + 2] + b0, acc[4 * j + 3] + b1);
+          } else {
+            // SiLU-gate: tile columns [0, BN/2) hold gate, [BN/2, BN) hold up for the same
+            // BN/2 output features (weights are interleaved per tile at load time).
+            const int ju = j + BN / 16;
+            float o[4];
 #pragma unroll
-          for (int h = 0; h < W; h += 16) {
-            if (c + h >= c_hi) break;
-            uint32_t g[16], u[16];
-            load_acc(c + h, g);
-            load_acc(H + c + h, u);
-#pragma unroll
-            for (int j = 0; j < 16; j += 8) {
-              float f[8];
-#pragma unroll
-              for (int e = 0; e < 8; ++e) {
-                const float gv = __uint_as_float(g[j + e]);
-                const float uv = __uint_as_float(u[j + e]);
-                f[e] = gv / (1.0f + __expf(-gv)) * uv;
-              }
-              stage_put((h + j) / 8, f);
+            for (int e = 0; e < 4; ++e) {
+              const float gv = acc[4 * j + e];
+              o[e] = gv / (1.0f + __expf(-gv)) * acc[4 * ju + e];
             }
+            stage_put(jj, 0, o[0], o[1]);
+            stage_put(jj, 1, o[2], o[3]);
           }
-          stage_flush(out_n0 + c, out_n0 + c_hi);
         }
+        stage_flush(out_n0 + cc, out_n0 + c_lo, out_n0 + c_hi);
       }
-      // release the accumulator buffer back to the MMA warp (split-K released it after the partial write)
-      if (split == 1) {
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tmem_empty[buf]);
-      } else {
+
+      if (split > 1) {
         // depart: the last slice to finish reading re-arms both counters for the next launch
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        if (warp == 2 && lane == 0) {
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+        if (ct == 0) {
           const uint32_t t = atomicAdd(p.tile_cnt + 2 * tile + 1, 1u);
           if (t == static_cast<uint32_t>(split - 1)) {
             p.tile_cnt[2 * tile] = 0u;
@@ -444,10 +383,10 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
       }
 
       if (p.rs_world > 0) {
-        // GEMM ⊕ reduce-scatter: all four epilogue warps have stored their rows; publish the
+        // GEMM ⊕ reduce-scatter: all eight consumer warps have stored their rows; publish the
         // tile to every owner rank whose rows it covers.
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        if (warp == 2 && lane == 0) {
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+        if (ct == 0) {
           __threadfence_system();
           const int m1 = min(m0 + kBlockM, p.M);
           const int o0 = p.rs_bcast ? 0 : m0 / p.rows_per_rank;
@@ -458,13 +397,6 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
         }
       }
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<1>(tmem_base, Cfg::kTmemCols);
   }
 }
 
@@ -511,9 +443,9 @@ static int pick_bn(int M, int N, int epi, int forced) {
   return best;
 }
 
-// Decode-sized M: few output tiles, so tile shape and a K split are chosen together. Cost model in SM clocks,
-// calibrated on B200 (profiles/gemm_splitk.md): a 64-deep k-block costs ~650 clk for BN=256 and ~420 clk for
-// BN<=128 (SMEM fill bound: 16 KB of A per k-block regardless of BN), a split-K round adds ~2000 + 24*BN.
+// Decode-sized M: few output tiles, so tile shape and a K split are chosen together. Cost model in SM clocks
+// (an estimate, not a measurement): a 64-deep k-block costs ~650 clk for BN=256 and ~420 clk for BN<=128 (SMEM
+// fill bound: 16 KB of A per k-block regardless of BN), a split-K round adds ~2000 + 24*BN.
 static void pick_split(int M, int N, int K, int epi, int forced_bn, int64_t ws_bytes, int max_tiles, int* bn_out,
                        int* split_out) {
   const int sms = num_sms();
@@ -526,7 +458,6 @@ static void pick_split(int M, int N, int K, int epi, int forced_bn, int64_t ws_b
     if (forced_bn > 0 && bn != forced_bn) continue;
     if (epi == kEpiSiluMul && bn < 64) continue;
     const int tiles = num_m * ((N + bn - 1) / bn);
-    // measured per-k-block time in SM clocks (benchmarks/gemm_tune.py, profiles/gemm_splitk.md)
     const double t_kb = bn >= 256 ? 650.0 : 420.0;
     for (int split = 1; split <= 8; split *= 2) {
       const int kpb = (num_kb + split - 1) / split;

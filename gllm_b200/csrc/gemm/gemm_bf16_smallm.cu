@@ -1,19 +1,17 @@
-// Small-M (decode) bf16 GEMM for sm_100a: swap-AB + split-K weight-streaming kernel.
+// Small-M (decode) bf16 GEMM for sm_90a: swap-AB + split-K weight-streaming kernel.
 //
 //     C[M, N] = A[M, K] · W[N, K]^T        with M <= 256 (a decode micro-batch)
 //
-// ncu on the 128xBN kernel (profiles/gemm_small_m_before.md) showed that for M << 128 the SM's
-// L2->SMEM fill bandwidth (~64 B/clk/SM) is spent on the 128-row activation tile that every CTA
-// re-reads, not on weights. Here the operands are swapped: the *weights* fill the 128-row MMA M
-// slot (every byte fetched is a weight byte that must come from HBM anyway) and the tokens sit in
-// the MMA N slot (N = BT = M rounded up to 16, runtime instruction descriptor), so one k-block
-// stage is 16 KB of weights + BT x 128 B of activations.  N/128 weight tiles are too few to fill
-// 148 SMs for the attention projections, so K is split S ways; partial tiles go to an fp32
-// workspace (L2 resident) and the last CTA to arrive for a tile reduces them in a fixed order
-// (deterministic), applies bias / SiLU-gate and stores bf16.
+// For M << 128 a 128 x BN tile spends the SM's L2->SMEM fill bandwidth on the 128-row activation tile that
+// every CTA re-reads, not on weights. Here the operands are swapped: the *weights* fill the 128-row MMA M
+// slot (every byte fetched is a weight byte that must come from HBM anyway) and the tokens sit in the MMA
+// N slot (N = BT = M rounded up to 16, 32, 64, 128 or 256), so one k-block stage is 16 KB of weights +
+// BT x 128 B of activations. N/128 weight tiles are too few to fill 132 SMs for the attention projections,
+// so K is split S ways; partial tiles go to an fp32 workspace (L2 resident) and the last CTA to arrive for
+// a tile reduces them in a fixed order (deterministic), applies bias / SiLU-gate and stores bf16.
 //
-// Same warp specialisation as gemm_bf16.cu: warp 0 TMA producer, warp 1 tcgen05.mma issuer,
-// warps 2-5 epilogue; TMEM accumulators double buffered.
+// Same warp specialisation as gemm_bf16.cu: warpgroup 0 TMA producer, warpgroups 1-2 wgmma (64 weight rows
+// each, accumulators in registers) and epilogue.
 #include <string.h>
 
 #include "../common/host_utils.h"
@@ -23,7 +21,8 @@ namespace b200 {
 
 static constexpr int kWTile = 128;  // weight rows per tile (MMA M)
 static constexpr int kBK = 64;
-static constexpr int kSmThreads = 192;
+static constexpr int kSmThreads = 384;
+static constexpr int kSmConsumers = 256;
 
 struct SmallMParams {
   int M, N, K, BT;  // BT: token tile (multiple of 16, >= M)
@@ -32,28 +31,25 @@ struct SmallMParams {
   __nv_bfloat16* C;
   int ldc;
   const __nv_bfloat16* bias;
-  float* ws;              // [num_n_tiles * S][128][BT] fp32 partials
+  float* ws;              // [num_n_tiles * S][BT][128] fp32 partials
   uint32_t* counters;     // [num_n_tiles], zero on entry, self-resetting
   int silu;               // 1: weight rows interleaved per 128: tile 2g = gate, tile 2g+1 = up
   int stages;
-  uint32_t tmem_cols;
 };
 
+template <int BT>
 __global__ void __launch_bounds__(kSmThreads, 1)
 gemm_smallm_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant__ CUtensorMap tmap_x,
                    const SmallMParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int S = p.stages;
-  const int w_bytes = kWTile * kBK * 2;
-  const int x_bytes = p.BT * kBK * 2;
-  const int stage_bytes = w_bytes + x_bytes;
+  constexpr int w_bytes = kWTile * kBK * 2;
+  constexpr int x_bytes = BT * kBK * 2;
+  constexpr int stage_bytes = w_bytes + x_bytes;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + S * stage_bytes);
   uint64_t* empty_bar = full_bar + S;
-  uint64_t* tmem_full = empty_bar + S;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-  uint32_t* flag_smem = tmem_ptr_smem + 1;
+  uint32_t* flag_smem = reinterpret_cast<uint32_t*>(empty_bar + S);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int num_n = (p.N + kWTile - 1) / kWTile;
@@ -65,23 +61,16 @@ gemm_smallm_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_cons
     tma_prefetch_desc(&tmap_x);
     for (int i = 0; i < S; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], 4);
+      mbar_init(&empty_bar[i], kSmConsumers / 32);
     }
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc<1>(tmem_ptr_smem, p.tmem_cols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
   griddep_launch();
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp < 4) {
+    regs_dealloc<40>();
+    if (warp == 0 && lane == 0) {
       uint32_t it = 0;
       // PDL: weight tiles of the first stages go in flight before waiting for the previous kernel
       uint32_t pre = 0;
@@ -117,95 +106,99 @@ gemm_smallm_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_cons
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc_bf16(kWTile, p.BT);
-      uint32_t it = 0, tcount = 0;
-      for (int u = blockIdx.x; u < num_units; u += gridDim.x, ++tcount) {
-        const int sp = u % p.S;
-        const int kb0 = sp * p.kb_per_split;
-        const int kb1 = min(kb0 + p.kb_per_split, num_kb);
-        const uint32_t buf = tcount & 1, aph = (tcount >> 1) & 1;
-        mbar_wait(&tmem_empty[buf], aph ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + buf * p.BT;
-        for (int kb = kb0; kb < kb1; ++kb, ++it) {
-          const int s = it % S;
-          const uint32_t ph = (it / S) & 1;
-          mbar_wait(&full_bar[s], ph);
-          tc_fence_after();
-          const uint32_t w_addr = smem_u32(smem + s * stage_bytes);
-          const uint64_t dw = make_sw128_kmajor_desc(w_addr);
-          const uint64_t dx = make_sw128_kmajor_desc(w_addr + w_bytes);
-#pragma unroll
-          for (int k = 0; k < kBK / 16; ++k) {
-            umma_bf16<1>(d_tmem, dw + (uint64_t)(k * 2), dx + (uint64_t)(k * 2), idesc, (kb > kb0 || k > 0) ? 1u : 0u);
-          }
-          umma_commit(&empty_bar[s]);
-        }
-        umma_commit(&tmem_full[buf]);
-      }
-    }
   } else {
-    // ===================== epilogue =====================
-    const int q = warp & 3;
-    const int et = q * 32 + lane;  // 0..127 : weight row inside the tile == TMEM lane
-    uint32_t tcount = 0;
+    // ===================== MMA + epilogue =====================
+    regs_alloc<232>();
+    griddep_wait();
+    const int ct = threadIdx.x - 128;      // 0..255
+    const int g = ct >> 7;                 // warpgroup: weight rows [64 g, 64 g + 64) of the tile
+    const int wq = (ct >> 5) & 3;
+    // accumulator fragment: acc[4 j + {0,1}] = (weight row e0, tokens 8 j + 2 (lane % 4) + {0,1}); +{2,3}: e0 + 8
+    const int e0 = 64 * g + 16 * wq + (lane >> 2);
+    const int mq = 2 * (lane & 3);
     const bool direct = (p.S == 1 && !p.silu);
-    for (int u = blockIdx.x; u < num_units; u += gridDim.x, ++tcount) {
-      const int nt = u / p.S;
-      const uint32_t buf = tcount & 1, aph = (tcount >> 1) & 1;
-      mbar_wait(&tmem_full[buf], aph);
-      tc_fence_after();
-      const uint32_t t_row = tmem_base + buf * p.BT + (static_cast<uint32_t>(q * 32) << 16);
-      const int n = nt * kWTile + et;
-      // partial tile in the workspace is token-major: ws[unit][m][128] -> every warp store is 128 B
-      float* __restrict__ wsu = p.ws + static_cast<size_t>(u) * p.BT * kWTile + et;
-      const float b = (direct && p.bias != nullptr && n < p.N) ? __bfloat162float(p.bias[n]) : 0.f;
-      for (int c = 0; c < p.BT; c += 16) {
-        uint32_t v[16];
-        tmem_ld_32x16(t_row + c, v);
-        tmem_ld_wait();
-        if (direct) {
-          if (n < p.N) {
+    uint32_t it = 0;
+    for (int u = blockIdx.x; u < num_units; u += gridDim.x) {
+      const int nt = u / p.S, sp = u % p.S;
+      const int kb0 = sp * p.kb_per_split;
+      const int kb1 = min(kb0 + p.kb_per_split, num_kb);
+      float acc[BT / 2];
 #pragma unroll
-            for (int j = 0; j < 16; ++j) {
-              const int m = c + j;
-              if (m < p.M) p.C[static_cast<size_t>(m) * p.ldc + n] = __float2bfloat16(__uint_as_float(v[j]) + b);
+      for (int i = 0; i < BT / 2; ++i) acc[i] = 0.f;
+      int prev_s = -1;
+      for (int kb = kb0; kb < kb1; ++kb, ++it) {
+        const int s = it % S;
+        mbar_wait(&full_bar[s], (it / S) & 1);
+        const uint32_t w_addr = smem_u32(smem + s * stage_bytes);
+        const uint64_t dw = make_sw128_kmajor_desc(w_addr + g * (64 * 128));
+        const uint64_t dx = make_sw128_kmajor_desc(w_addr + w_bytes);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kBK / 16; ++k)
+          wgmma_bf16_ss<BT>(acc, dw + (uint64_t)(k * 2), dx + (uint64_t)(k * 2), (kb > kb0 || k > 0) ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev_s >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_s]);
+        prev_s = s;
+      }
+      wgmma_wait<0>();
+      reg_fence(acc);
+      if (prev_s >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_s]);
+
+      if (direct) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int n = nt * kWTile + e0 + 8 * h;
+          if (n >= p.N) continue;
+          const float b = p.bias != nullptr ? __bfloat162float(p.bias[n]) : 0.f;
+#pragma unroll
+          for (int j = 0; j < BT / 8; ++j) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int m = 8 * j + mq + e;
+              if (m < p.M) p.C[static_cast<size_t>(m) * p.ldc + n] = __float2bfloat16(acc[4 * j + 2 * h + e] + b);
             }
           }
-        } else {
+        }
+        continue;
+      }
+      // partial tile in the workspace is token-major: ws[unit][m][128]
+      float* __restrict__ wsu = p.ws + static_cast<size_t>(u) * BT * kWTile + e0;
 #pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            if (c + j < p.M) wsu[static_cast<size_t>(c + j) * kWTile] = __uint_as_float(v[j]);
+      for (int j = 0; j < BT / 8; ++j) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int m = 8 * j + mq + e;
+          if (m < p.M) {
+            wsu[static_cast<size_t>(m) * kWTile] = acc[4 * j + e];
+            wsu[static_cast<size_t>(m) * kWTile + 8] = acc[4 * j + 2 + e];
           }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[buf]);
-      if (direct) continue;
 
       // publish the partial tile; the last split to arrive reduces (fixed order => deterministic)
       __threadfence();
-      asm volatile("bar.sync 1, 128;" ::: "memory");
+      asm volatile("bar.sync 1, 256;" ::: "memory");
       // SiLU-gate: weight rows are interleaved per 128 (tile 2g = gate, tile 2g+1 = up of the same 128
       // features), so a *pair* of tiles (2 S units) completes one output group.
       const int grp = p.silu ? (nt >> 1) : nt;
       const uint32_t need = static_cast<uint32_t>(p.silu ? 2 * p.S : p.S);
-      if (et == 0) {
+      if (ct == 0) {
         const uint32_t old = atomicAdd(p.counters + grp, 1u);
         *flag_smem = (old == need - 1u) ? 1u : 0u;
       }
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      if (*flag_smem) {
+      asm volatile("bar.sync 1, 256;" ::: "memory");
+      const uint32_t last = *flag_smem;
+      asm volatile("bar.sync 1, 256;" ::: "memory");   // flag read by all before the next unit rewrites it
+      if (last) {
         __threadfence();
         const float* __restrict__ base =
-            p.ws + static_cast<size_t>(p.silu ? 2 * grp : nt) * p.S * p.BT * kWTile;
-        const size_t unit_stride = static_cast<size_t>(p.BT) * kWTile;
-        const int n4 = et & 31;   // float4 column group
-        const int mr = et >> 5;   // 0..3
-        constexpr int U = 4;      // rows in flight per thread
+            p.ws + static_cast<size_t>(p.silu ? 2 * grp : nt) * p.S * BT * kWTile;
+        const size_t unit_stride = static_cast<size_t>(BT) * kWTile;
+        const int n4 = ct & 31;   // float4 column group
+        const int mr = ct >> 5;   // 0..7
+        constexpr int U = 2;      // rows in flight per thread
+        constexpr int RS = 8;     // rows per pass of the 256 threads
         if (!p.silu) {
           const int ncol = nt * kWTile + n4 * 4;
           float bb[4] = {0.f, 0.f, 0.f, 0.f};
@@ -213,30 +206,30 @@ gemm_smallm_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_cons
 #pragma unroll
             for (int j = 0; j < 4; ++j) if (ncol + j < p.N) bb[j] = __bfloat162float(p.bias[ncol + j]);
           }
-          for (int m0 = 0; m0 < p.M; m0 += 4 * U) {
-            float4 acc[U];
+          for (int m0 = 0; m0 < p.M; m0 += RS * U) {
+            float4 a[U];
 #pragma unroll
             for (int uu = 0; uu < U; ++uu) {
-              const int m = m0 + uu * 4 + mr;
-              acc[uu] = make_float4(bb[0], bb[1], bb[2], bb[3]);
+              const int m = m0 + uu * RS + mr;
+              a[uu] = make_float4(bb[0], bb[1], bb[2], bb[3]);
               if (m < p.M) {
                 for (int s2 = 0; s2 < p.S; ++s2) {
                   const float4 t = __ldcg(reinterpret_cast<const float4*>(
                       base + s2 * unit_stride + static_cast<size_t>(m) * kWTile + n4 * 4));
-                  acc[uu].x += t.x; acc[uu].y += t.y; acc[uu].z += t.z; acc[uu].w += t.w;
+                  a[uu].x += t.x; a[uu].y += t.y; a[uu].z += t.z; a[uu].w += t.w;
                 }
               }
             }
 #pragma unroll
             for (int uu = 0; uu < U; ++uu) {
-              const int m = m0 + uu * 4 + mr;
+              const int m = m0 + uu * RS + mr;
               if (m < p.M) {
                 __nv_bfloat16* dst = p.C + static_cast<size_t>(m) * p.ldc + ncol;
                 if (ncol + 3 < p.N) {
-                  *reinterpret_cast<uint2*>(dst) = make_uint2(pack_bf16(acc[uu].x, acc[uu].y), pack_bf16(acc[uu].z, acc[uu].w));
+                  *reinterpret_cast<uint2*>(dst) = make_uint2(pack_bf16(a[uu].x, a[uu].y), pack_bf16(a[uu].z, a[uu].w));
                 } else {
-                  const float a[4] = {acc[uu].x, acc[uu].y, acc[uu].z, acc[uu].w};
-                  for (int j = 0; j < 4; ++j) if (ncol + j < p.N) dst[j] = __float2bfloat16(a[j]);
+                  const float v[4] = {a[uu].x, a[uu].y, a[uu].z, a[uu].w};
+                  for (int j = 0; j < 4; ++j) if (ncol + j < p.N) dst[j] = __float2bfloat16(v[j]);
                 }
               }
             }
@@ -245,48 +238,53 @@ gemm_smallm_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_cons
           // gate partials live in the units of tile 2g, up partials in the units of tile 2g+1
           const int f = grp * kWTile + n4 * 4;
           const float* __restrict__ base_up = base + static_cast<size_t>(p.S) * unit_stride;
-          for (int m0 = 0; m0 < p.M; m0 += 4 * U) {
-            float4 g[U], up[U];
+          for (int m0 = 0; m0 < p.M; m0 += RS * U) {
+            float4 gg[U], up[U];
 #pragma unroll
             for (int uu = 0; uu < U; ++uu) {
-              const int m = m0 + uu * 4 + mr;
-              g[uu] = make_float4(0.f, 0.f, 0.f, 0.f);
-              up[uu] = g[uu];
+              const int m = m0 + uu * RS + mr;
+              gg[uu] = make_float4(0.f, 0.f, 0.f, 0.f);
+              up[uu] = gg[uu];
               if (m < p.M) {
                 for (int s2 = 0; s2 < p.S; ++s2) {
                   const size_t off = s2 * unit_stride + static_cast<size_t>(m) * kWTile + n4 * 4;
                   const float4 tg = __ldcg(reinterpret_cast<const float4*>(base + off));
                   const float4 tu = __ldcg(reinterpret_cast<const float4*>(base_up + off));
-                  g[uu].x += tg.x; g[uu].y += tg.y; g[uu].z += tg.z; g[uu].w += tg.w;
+                  gg[uu].x += tg.x; gg[uu].y += tg.y; gg[uu].z += tg.z; gg[uu].w += tg.w;
                   up[uu].x += tu.x; up[uu].y += tu.y; up[uu].z += tu.z; up[uu].w += tu.w;
                 }
               }
             }
 #pragma unroll
             for (int uu = 0; uu < U; ++uu) {
-              const int m = m0 + uu * 4 + mr;
+              const int m = m0 + uu * RS + mr;
               if (m < p.M && f + 3 < p.N / 2) {
-                const float o0 = g[uu].x / (1.f + __expf(-g[uu].x)) * up[uu].x;
-                const float o1 = g[uu].y / (1.f + __expf(-g[uu].y)) * up[uu].y;
-                const float o2 = g[uu].z / (1.f + __expf(-g[uu].z)) * up[uu].z;
-                const float o3 = g[uu].w / (1.f + __expf(-g[uu].w)) * up[uu].w;
+                const float o0 = gg[uu].x / (1.f + __expf(-gg[uu].x)) * up[uu].x;
+                const float o1 = gg[uu].y / (1.f + __expf(-gg[uu].y)) * up[uu].y;
+                const float o2 = gg[uu].z / (1.f + __expf(-gg[uu].z)) * up[uu].z;
+                const float o3 = gg[uu].w / (1.f + __expf(-gg[uu].w)) * up[uu].w;
                 *reinterpret_cast<uint2*>(p.C + static_cast<size_t>(m) * p.ldc + f) =
                     make_uint2(pack_bf16(o0, o1), pack_bf16(o2, o3));
               }
             }
           }
         }
-        if (et == 0) p.counters[grp] = 0u;  // ready for the next launch
+        if (ct == 0) p.counters[grp] = 0u;  // ready for the next launch
       }
     }
   }
+}
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<1>(tmem_base, p.tmem_cols);
+template <int BT>
+static int launch_smallm(const CUtensorMap& tw, const CUtensorMap& tx, const SmallMParams& p, int grid, int smem_bytes,
+                         cudaStream_t st) {
+  static PerDeviceOnce configured;
+  if (configured.need()) {
+    CUDA_CHECK_RET(cudaFuncSetAttribute(gemm_smallm_kernel<BT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    configured.done();
   }
+  CUDA_CHECK_RET(launch_pdl(gemm_smallm_kernel<BT>, dim3(grid), dim3(kSmThreads), smem_bytes, st, tw, tx, p));
+  return 0;
 }
 
 }  // namespace b200
@@ -306,7 +304,7 @@ GLLM_EXPORT int gllm_gemm_smallm(const void* A, int64_t lda, const void* W, int6
   SmallMParams p;
   memset(&p, 0, sizeof(p));
   p.M = M; p.N = N; p.K = K;
-  p.BT = ((M + 15) / 16) * 16;
+  p.BT = M <= 16 ? 16 : M <= 32 ? 32 : M <= 64 ? 64 : M <= 128 ? 128 : 256;  // wgmma N of the token tile
   const int num_n = (N + kWTile - 1) / kWTile;
   const int num_kb = (K + kBK - 1) / kBK;
   const int sms = num_sms();
@@ -321,7 +319,7 @@ GLLM_EXPORT int gllm_gemm_smallm(const void* A, int64_t lda, const void* W, int6
     const int waves = (units + sms - 1) / sms;
     // unit of cost = one k-block of this shape (fill-bound: (16 KB + BT*128 B) / 64 B/clk)
     const double kb_cyc = 256.0 + 2.0 * p.BT;
-    const double ovh = 2.0 + 30.0 * p.BT / kb_cyc;                // prologue + TMEM drain/store per unit
+    const double ovh = 2.0 + 30.0 * p.BT / kb_cyc;                // prologue + accumulator drain/store per unit
     const double red = (s > 1) ? 4.0 * M * s / kb_cyc : 0.0;      // last-arriver reduction
     const double cost = waves * (kbs + ovh) + red;
     if (cost < best_cost - 1e-9) { best_cost = cost; best_s = s; }
@@ -347,21 +345,18 @@ GLLM_EXPORT int gllm_gemm_smallm(const void* A, int64_t lda, const void* W, int6
   int stages = (216 * 1024) / stage_bytes;
   if (stages > 12) stages = 12;
   p.stages = stages;
-  uint32_t cols = 32;
-  while (cols < static_cast<uint32_t>(2 * p.BT)) cols *= 2;
-  p.tmem_cols = cols;
   const int smem_bytes = stages * stage_bytes + 1024 + 512;
   CUtensorMap tw, tx;
   if (make_tmap_2d(&tw, W, N, K, ldw * 2, kWTile, kBK, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16)) return 1;
   if (make_tmap_2d(&tx, A, M, K, lda * 2, p.BT, kBK, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16)) return 1;
-  static PerDeviceOnce configured;
-  if (configured.need()) {
-    CUDA_CHECK_RET(cudaFuncSetAttribute(gemm_smallm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    configured.done();
-  }
   const int units = num_n * p.S;
   const int grid = units < sms ? units : sms;
-  CUDA_CHECK_RET(launch_pdl(gemm_smallm_kernel, dim3(grid), dim3(kSmThreads), smem_bytes,
-                            reinterpret_cast<cudaStream_t>(stream), tw, tx, p));
-  return 0;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  switch (p.BT) {
+    case 16: return launch_smallm<16>(tw, tx, p, grid, smem_bytes, st);
+    case 32: return launch_smallm<32>(tw, tx, p, grid, smem_bytes, st);
+    case 64: return launch_smallm<64>(tw, tx, p, grid, smem_bytes, st);
+    case 128: return launch_smallm<128>(tw, tx, p, grid, smem_bytes, st);
+    default: return launch_smallm<256>(tw, tx, p, grid, smem_bytes, st);
+  }
 }

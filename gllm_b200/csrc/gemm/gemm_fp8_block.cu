@@ -1,4 +1,4 @@
-// Block-scaled FP8 (e4m3) GEMM for sm_100a, DeepSeek-V3 / Qwen3-FP8 checkpoint semantics
+// Block-scaled FP8 (e4m3) GEMM for sm_90a, DeepSeek-V3 / Qwen3-FP8 checkpoint semantics
 // (reference: gllm/layers/quantization/fp8.py:54-250 — Triton w8a8_block_fp8_matmul):
 //
 //   C[M,N] = sum_kb  (A8[M, kb] · W8[N, kb]^T) * a_s[M, kb] * w_s[N/128, kb]      (+ bias) -> bf16
@@ -6,12 +6,11 @@
 //       (stored K-block-major so a warp's 32 rows read 32 consecutive floats)
 //   W8: weights e4m3 [N, K] with fp32 scales per 128x128 block, w_s [N/128, K/128]
 //
-// The checkpoint scales are arbitrary fp32 values (not the power-of-two UE8M0 factors that
-// `kind::mxf8f6f4.block_scale` applies in hardware), so each 128-deep K block is multiplied by
-// `tcgen05.mma.kind::f8f6f4` into its own TMEM buffer (4 MMAs of K=32, the first one overwriting)
-// and the epilogue warps promote it: acc += partial * a_s[row] * w_s[tile] in fp32 registers. Two
-// TMEM buffers ping-pong per K block so the tensor core runs block kb+1 while the CUDA cores fold
-// block kb. Same TMA (SWIZZLE_128B, 128 fp8 = one 128-byte row) / mbarrier ring as gemm_bf16.cu.
+// The checkpoint scales are arbitrary fp32 values, so each 128-deep K block is multiplied by
+// `wgmma.mma_async ... e4m3.e4m3` into its own register accumulator (4 MMAs of K=32, the first one
+// overwriting) and then promoted: acc += partial * a_s[row] * w_s[tile] in fp32 registers. Two consumer
+// warpgroups own 64 rows each of the 128 x 128 tile. Same TMA (SWIZZLE_128B, 128 fp8 = one 128-byte row) /
+// mbarrier ring as gemm_bf16.cu.
 //
 // Also here: the dynamic per-token-group activation quantiser (reference fp8.py:354-552).
 #include <cuda_fp8.h>
@@ -24,7 +23,7 @@ namespace b200 {
 
 static constexpr int kFBM = 128, kFBN = 128, kFBK = 128;  // K block = 128 fp8 = 128 B
 static constexpr int kFStages = 6;
-static constexpr int kFThreads = 192;
+static constexpr int kFThreads = 384;  // warpgroup 0: TMA producer, warpgroups 1-2: MMA + epilogue
 
 struct Fp8Params {
   int M, N, K;
@@ -51,9 +50,6 @@ gemm_fp8_block_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_c
   constexpr int kABytes = kFBM * kFBK, kBBytes = kFBN * kFBK, kStageBytes = kABytes + kBBytes;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kFStages * kStageBytes);
   uint64_t* empty_bar = full_bar + kFStages;
-  uint64_t* tmem_full = empty_bar + kFStages;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(tmem_empty + 2);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const bool grouped = p.tile_expert != nullptr;
@@ -66,18 +62,14 @@ gemm_fp8_block_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_c
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_b);
-    for (int i = 0; i < kFStages; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&tmem_full[i], 1); mbar_init(&tmem_empty[i], 4); }
+    for (int i = 0; i < kFStages; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 8); }
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc<1>(tmem_ptr_smem, 256);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp < 4) {
+    regs_dealloc<40>();
+    if (warp == 0 && lane == 0) {
       uint32_t it = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const int m0 = (tile % num_m) * kFBM, n0 = (tile / num_m) * kFBN;
@@ -92,108 +84,89 @@ gemm_fp8_block_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_c
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc_e4m3(kFBM, kFBN);
-      uint32_t it = 0;  // global k-block counter == TMEM hand-off counter
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        for (int kb = 0; kb < num_kb; ++kb, ++it) {
-          const int s = it % kFStages;
-          const uint32_t buf = it & 1;
-          mbar_wait(&tmem_empty[buf], ((it >> 1) & 1) ^ 1);
-          mbar_wait(&full_bar[s], (it / kFStages) & 1);
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(smem + s * kStageBytes);
-          const uint64_t da = make_sw128_kmajor_desc(a_addr);
-          const uint64_t db = make_sw128_kmajor_desc(a_addr + kABytes);
-          const uint32_t d_tmem = tmem_base + buf * kFBN;
-#pragma unroll
-          for (int k = 0; k < kFBK / 32; ++k)  // UMMA K = 32 for 8-bit operands: +32 B per step
-            umma_f8(d_tmem, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), idesc, k > 0 ? 1u : 0u);
-          umma_commit(&empty_bar[s]);
-          umma_commit(&tmem_full[buf]);
-        }
-      }
-    }
   } else {
-    const int q = warp & 3;
+    regs_alloc<232>();
+    const int ct = threadIdx.x - 128;
+    const int g = ct >> 7, wq = (ct >> 5) & 3;
+    const int r_in = 64 * g + 16 * wq + (lane >> 2);   // rows r_in and r_in + 8 of the tile
+    const int cq = 2 * (lane & 3);                     // columns 8 j + cq + {0, 1}
     uint32_t it = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int m0 = (tile % num_m) * kFBM, n0 = (tile / num_m) * kFBN;
-      const int row = m0 + q * 32 + lane;
-      const bool row_ok = row < p.M;
-      float acc[kFBN];
+      const int row0 = m0 + r_in, row1 = row0 + 8;
+      float acc[kFBN / 2], part[kFBN / 2];
 #pragma unroll
-      for (int i = 0; i < kFBN; ++i) acc[i] = 0.f;
+      for (int i = 0; i < kFBN / 2; ++i) acc[i] = 0.f;
       for (int kb = 0; kb < num_kb; ++kb, ++it) {
-        const uint32_t buf = it & 1;
-        const float sa = row_ok ? p.a_s[static_cast<size_t>(kb) * p.lda_s + row] : 0.f;
-        float sc, sc_hi;
+        const int s = it % kFStages;
+        mbar_wait(&full_bar[s], (it / kFStages) & 1);
+        const uint32_t a_addr = smem_u32(smem + s * kStageBytes);
+        const uint64_t da = make_sw128_kmajor_desc(a_addr + g * (64 * 128));
+        const uint64_t db = make_sw128_kmajor_desc(a_addr + kABytes);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kFBK / 32; ++k)  // K = 32 for 8-bit operands: +32 B per step
+          wgmma_e4m3_ss<kFBN>(part, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), k > 0 ? 1u : 0u);
+        wgmma_commit();
+        // scales of this K block load while the tensor core runs
+        const float sa0 = row0 < p.M ? p.a_s[static_cast<size_t>(kb) * p.lda_s + row0] : 0.f;
+        const float sa1 = row1 < p.M ? p.a_s[static_cast<size_t>(kb) * p.lda_s + row1] : 0.f;
+        float sw, sw_hi;
         if (grouped) {
           const float* ws = p.w_s + static_cast<size_t>(p.tile_expert[tile % num_m]) * p.ws_stride_e +
                             static_cast<size_t>(n0 / 64) * num_kb + kb;
-          sc = sa * ws[0];
-          sc_hi = sa * ws[num_kb];
+          sw = ws[0];
+          sw_hi = ws[num_kb];
         } else {
-          sc = sc_hi = sa * p.w_s[static_cast<size_t>(n0 / kFBN) * num_kb + kb];
+          sw = sw_hi = p.w_s[static_cast<size_t>(n0 / kFBN) * num_kb + kb];
         }
-        mbar_wait(&tmem_full[buf], (it >> 1) & 1);
-        tc_fence_after();
-        const uint32_t t_row = tmem_base + buf * kFBN + (static_cast<uint32_t>(q * 32) << 16);
+        wgmma_wait<0>();
+        reg_fence(part);
+        if (lane == 0) mbar_arrive(&empty_bar[s]);
 #pragma unroll
-        for (int c = 0; c < kFBN; c += 32) {
-          uint32_t v[32];
-          tmem_ld_32x32(t_row + c, v);
-          tmem_ld_wait();
-#pragma unroll
-          for (int j = 0; j < 32; ++j) acc[c + j] = fmaf(__uint_as_float(v[j]), c < 64 ? sc : sc_hi, acc[c + j]);
+        for (int j = 0; j < kFBN / 8; ++j) {
+          const float w = j < 8 ? sw : sw_hi;   // columns < 64 / >= 64
+          acc[4 * j] = fmaf(part[4 * j], sa0 * w, acc[4 * j]);
+          acc[4 * j + 1] = fmaf(part[4 * j + 1], sa0 * w, acc[4 * j + 1]);
+          acc[4 * j + 2] = fmaf(part[4 * j + 2], sa1 * w, acc[4 * j + 2]);
+          acc[4 * j + 3] = fmaf(part[4 * j + 3], sa1 * w, acc[4 * j + 3]);
         }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tmem_empty[buf]);
       }
-      if (row_ok && p.silu) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int row = h ? row1 : row0;
+        if (row >= p.M) continue;
         __nv_bfloat16* crow = p.C + static_cast<size_t>(row) * p.ldc;
+        if (p.silu) {
 #pragma unroll
-        for (int c = 0; c < 64; c += 8) {
-          const int col = n0 / 2 + c;
-          if (col < p.N / 2) {
-            float f[8];
+          for (int j = 0; j < 8; ++j) {
+            const int col = n0 / 2 + 8 * j + cq;
+            if (col < p.N / 2) {
+              float f[2];
 #pragma unroll
-            for (int e = 0; e < 8; ++e) {
-              const float gv = acc[c + e];
-              f[e] = gv / (1.0f + __expf(-gv)) * acc[64 + c + e];
+              for (int e = 0; e < 2; ++e) {
+                const float gv = acc[4 * j + 2 * h + e];
+                f[e] = gv / (1.0f + __expf(-gv)) * acc[4 * (j + 8) + 2 * h + e];
+              }
+              *reinterpret_cast<uint32_t*>(crow + col) = pack_bf16(f[0], f[1]);
             }
-            st_v4(crow + col, make_uint4(pack_bf16(f[0], f[1]), pack_bf16(f[2], f[3]), pack_bf16(f[4], f[5]),
-                                         pack_bf16(f[6], f[7])));
           }
-        }
-      } else if (row_ok) {
-        __nv_bfloat16* crow = p.C + static_cast<size_t>(row) * p.ldc;
+        } else {
 #pragma unroll
-        for (int c = 0; c < kFBN; c += 8) {
-          const int col = n0 + c;
-          if (col < p.N) {
-            float f[8];
-#pragma unroll
-            for (int e = 0; e < 8; ++e) f[e] = acc[c + e];
-            if (p.bias != nullptr) {
-              const uint4 bv = *reinterpret_cast<const uint4*>(p.bias + col);
-              const float2 b0 = unpack_bf16(bv.x), b1 = unpack_bf16(bv.y), b2 = unpack_bf16(bv.z), b3 = unpack_bf16(bv.w);
-              f[0] += b0.x; f[1] += b0.y; f[2] += b1.x; f[3] += b1.y; f[4] += b2.x; f[5] += b2.y; f[6] += b3.x; f[7] += b3.y;
+          for (int j = 0; j < kFBN / 8; ++j) {
+            const int col = n0 + 8 * j + cq;
+            if (col < p.N) {
+              float f0 = acc[4 * j + 2 * h], f1 = acc[4 * j + 2 * h + 1];
+              if (p.bias != nullptr) {
+                const float2 bv = unpack_bf16(*reinterpret_cast<const uint32_t*>(p.bias + col));
+                f0 += bv.x; f1 += bv.y;
+              }
+              *reinterpret_cast<uint32_t*>(crow + col) = pack_bf16(f0, f1);
             }
-            st_v4(crow + col, make_uint4(pack_bf16(f[0], f[1]), pack_bf16(f[2], f[3]), pack_bf16(f[4], f[5]),
-                                         pack_bf16(f[6], f[7])));
           }
         }
       }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<1>(tmem_base, 256);
   }
 }
 

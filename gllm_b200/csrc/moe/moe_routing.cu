@@ -1,4 +1,4 @@
-// MoE routing + token permutation kernels for sm_100a.
+// MoE routing + token permutation kernels for sm_90a.
 //
 //   topk_softmax      softmax over experts + top-k (+renorm)            (ref: vLLM _moe_C.topk_softmax,
 //                                                                         gllm/layers/moe/topk.py:141-171)
@@ -10,7 +10,7 @@
 //   moe_gather        xs[row] = x[token(row)]  (rows of padding are zero)
 //   moe_combine       out[t] = sum_j w[t,j] * y[pos[t,j]]   (ref: moe_sum, fused with the routing weight)
 //
-// The expert GEMMs themselves are the tcgen05 kernel in gemm/gemm_bf16.cu running in grouped mode
+// The expert GEMMs themselves are the wgmma kernel in gemm/gemm_bf16.cu running in grouped mode
 // (per-M-tile expert id selects the weight slab; the tile count is read from device memory so the
 // whole MoE block is CUDA-graph capturable without a host sync).
 #include "../common/host_utils.h"

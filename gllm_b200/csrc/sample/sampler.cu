@@ -1,4 +1,4 @@
-// Fused sampling for sm_100a: repetition penalty -> temperature -> top-k -> top-p -> draw.
+// Fused sampling for sm_90a: repetition penalty -> temperature -> top-k -> top-p -> draw.
 //
 // The reference does this with ~15 PyTorch ops including a full-vocabulary sort
 // (gllm/layers/sampler.py:8-54). Here one CTA per sequence makes a handful of passes over its

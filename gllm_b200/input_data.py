@@ -351,7 +351,7 @@ class InputData:
         self._put(self._qsl, batch.query_start_loc)
         if self.num_emit:
             self._put(self._logits_idx, batch.logits_idx)
-            # the greedy argmax path of the sm_100a sampler reads none of these
+            # the greedy argmax path of the sm_90a sampler reads none of these
             if not (self.device.type == "cuda" and batch.all_greedy and not batch.need_penalty):
                 self._put(self._temperature, batch.temperature)
                 self._put(self._top_k, batch.top_k)

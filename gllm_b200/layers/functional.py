@@ -1,6 +1,6 @@
 """Device-directed op entry points used by the model code.
 
-CUDA tensors always run the hand-written sm_100a kernels (`ops.sm100`); CPU tensors run the
+CUDA tensors always run the hand-written sm_90a kernels (`ops.sm100`); CPU tensors run the
 PyTorch oracle (`ops.ref`) — that is the CPU plumbing/test path only, never a GPU fallback.
 """
 from __future__ import annotations

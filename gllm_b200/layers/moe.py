@@ -7,7 +7,7 @@ rank holds all experts with `intermediate / tp` columns. The block returns the *
 this rank's experts; the caller reduces it over the TP group together with the following
 residual-add + RMSNorm (`TPComm.reduce_add_norm`).
 
-On CUDA the experts run as one grouped tcgen05 GEMM pair over expert-sorted token slots
+On CUDA the experts run as one grouped wgmma GEMM pair over expert-sorted token slots
 (csrc/moe/); the all-to-all dispatch/combine variant lives in parallel/fused.py.
 """
 from __future__ import annotations
@@ -73,7 +73,7 @@ class FusedMoE(nn.Module):
 
     # -- routing ----------------------------------------------------------------------------------
     def process_weights(self):
-        """The tcgen05 GEMM wants N % 8 == 0: expert counts like 60 (Qwen1.5-MoE) get a zero-padded router
+        """The wgmma GEMM wants N % 8 == 0: expert counts like 60 (Qwen1.5-MoE) get a zero-padded router
         weight, built once after loading (before CUDA-graph capture); the logits are sliced back to E columns."""
         if self.router_w.is_cuda and self.num_experts % 8 != 0:
             e_pad = (self.num_experts + 7) // 8 * 8
@@ -141,7 +141,7 @@ class FusedMoE(nn.Module):
             return
         if self.w13.is_cuda:
             # the grouped GEMM's SiLU-gate epilogue wants gate/up rows interleaved per 64
-            assert self.inter % 64 == 0, "sm_100a MoE path needs intermediate % 64 == 0"
+            assert self.inter % 64 == 0, "sm_90a MoE path needs intermediate % 64 == 0"
             gu = ref.interleave_gate_up(gu, 64)
         self.w13.data[le].copy_(gu)
         self.w2.data[le].copy_(down)

@@ -4,10 +4,10 @@
 MLA here stores the *latent* KV cache — `[kv_c (kv_lora_rank, RMS-normed) | k_pe (rope dims, rotated)]`
 per token, one "head", replicated on every TP rank (like the reference's MLA `Segment`,
 gllm/memory_manager.py:38-42) — and q heads are split over TP. Routing uses the group-limited top-k
-kernel (sigmoid + bias-corrected `noaux_tc` for V3), experts run through the grouped tcgen05 GEMMs,
+kernel (sigmoid + bias-corrected `noaux_tc` for V3), experts run through the grouped wgmma GEMMs,
 shared experts are an ordinary gated MLP whose partial output is reduced together with the routed one.
 
-On sm_100a the attention runs in the *absorbed* form: q_nope·W_UK per head (batched tcgen05 GEMM over strided
+On sm_90a the attention runs in the *absorbed* form: q_nope·W_UK per head (batched wgmma GEMM over strided
 views, written straight into the 576-wide query), fused RoPE + latent-cache write, split-KV multi-query attention
 over the paged latent cache (csrc/attn/mla_attention.cu), then out_lat·W_UV per head (the same batched GEMM,
 written in the [T, heads·v] layout o_proj reads). No cuBLAS and no host synchronisation on that path, so decode
@@ -138,7 +138,7 @@ class MLAAttention(nn.Module):
         return self._w_abs
 
     def _forward_absorbed(self, inp, q, kv_c, k_pe, cache):
-        """sm_100a path: multi-query attention over the latent cache (csrc/attn/mla_attention.cu). No host
+        """sm_90a path: multi-query attention over the latent cache (csrc/attn/mla_attention.cu). No host
         synchronisation, so decode batches run inside CUDA graphs."""
         from gllm_b200.ops import sm100
         t, hl = q.shape[0], self.num_heads

@@ -1,7 +1,7 @@
 """Op namespace.
 
 `gllm_b200.ops.ref`   — pure-PyTorch oracle (CPU-capable; tests + CPU plumbing).
-`gllm_b200.ops.sm100` — the product: hand-written sm_100a kernels.
+`gllm_b200.ops.sm100` — the product: hand-written sm_90a kernels.
 
 `backend()` picks sm100 whenever a CUDA device is present; there is no silent fallback —
 if the kernel library cannot be loaded on a GPU box, importing the ops raises.

@@ -1,7 +1,7 @@
-"""ctypes binding to the in-tree sm_100a kernel library.
+"""ctypes binding to the in-tree sm_90a kernel library.
 
 The library is `gllm_b200/_C/libgllm_b200.so`, built by `gllm_b200.build` with plain
-nvcc (`-gencode arch=compute_100a,code=sm_100a`). It exposes a flat C ABI; every entry
+nvcc (`-gencode arch=compute_90a,code=sm_90a`). It exposes a flat C ABI; every entry
 point takes raw device pointers plus the CUDA stream handle and returns 0 on success.
 
 On a GPU box a missing library is a hard error (we never silently fall back to PyTorch

@@ -1,6 +1,6 @@
 """Pure-PyTorch reference implementations of every op (CPU-capable).
 
-These are the correctness oracle for the sm_100a kernels (tests compare against them in
+These are the correctness oracle for the sm_90a kernels (tests compare against them in
 fp32) and the execution path for the CPU plumbing tests (BASELINE config #1: scheduler +
 paged-KV on CPU). They are NOT a product path: on a GPU box the engine always runs the
 hand-written kernels in `gllm_b200.ops.sm100`.

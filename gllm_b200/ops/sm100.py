@@ -1,4 +1,4 @@
-"""Python front-ends of the hand-written sm_100a kernels (ctypes -> libgllm_b200.so).
+"""Python front-ends of the hand-written sm_90a kernels (ctypes -> libgllm_b200.so).
 
 Each function validates shapes/dtypes, allocates the output and launches on the current
 CUDA stream. No fallback: if the library is missing on a GPU box this raises.
@@ -15,7 +15,7 @@ from gllm_b200.ops import lib as _lib
 from gllm_b200.ops.lib import GemmComm, check, stream_ptr
 
 _BF16 = torch.bfloat16
-NUM_SMS = 148
+NUM_SMS = 132   # H100 SXM
 
 
 def _p(t: Optional[torch.Tensor]):
@@ -40,7 +40,6 @@ def _count(n=1):
 # ----------------------------------------------------------------------------------------------
 _FORCE_BN = int(os.environ.get("GLLM_GEMM_BN", "0"))
 _SMALLM_MAX = int(os.environ.get("GLLM_GEMM_SMALLM_MAX", "32"))   # M <= this -> swap-AB split-K kernel
-# (measured crossover vs the 128xBN kernel on B200: profiles/gemm_smallm.md)
 _FORCE_SPLIT = int(os.environ.get("GLLM_GEMM_SPLIT", "0"))
 _SMALLM_WS_FLOATS = 24 << 20   # fp32 partial-sum workspace shared by the swap-AB and the split-K kernels
 _SPLITK_MAX_TILES = 4096
@@ -225,10 +224,9 @@ def rope_kv_write(q: torch.Tensor, k: torch.Tensor, v: Optional[torch.Tensor], p
 # ----------------------------------------------------------------------------------------------
 _attn_ws = {}
 _FUSED_MERGE = os.environ.get("GLLM_ATTN_FUSED_MERGE", "0") == "1"
-# tcgen05 / TMEM prefill attention (csrc/attn/prefill_attention_tc.cu) is the default prefill kernel (validated on
-# B200: profiles/attn_prefill_tc.md; 1.3-2.1x the mma.sync kernel); GLLM_ATTN_TC=0 selects the mma.sync kernel, which
-# also serves the shapes outside the tcgen05 kernel's envelope. ATTN_TC_KV = keys per pipeline stage (64 or 128;
-# 64 measured faster at every shape). Module attributes so tests / benches can flip them.
+# wgmma prefill attention (csrc/attn/prefill_attention_tc.cu) is the default prefill kernel; GLLM_ATTN_TC=0 selects
+# the mma.sync kernel, which also serves the shapes outside the wgmma kernel's envelope. ATTN_TC_KV = keys per
+# pipeline stage (64 or 128). Module attributes so tests / benches can flip them.
 ATTN_TC = os.environ.get("GLLM_ATTN_TC", "1") == "1"
 ATTN_TC_KV = int(os.environ.get("GLLM_ATTN_TC_KV", "64"))
 
@@ -318,7 +316,7 @@ def paged_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tenso
             rc = L.gllm_attn_prefill_tc(_p(q), q.stride(0), _p(out), _p(k_cache), _p(v_cache), pages, _p(block_table),
                                         _p(seq_lens), _p(query_start_loc), n_prefill, num_decode_seqs, max_q_len,
                                         max_blocks, hq, hkv, d, page_size, float(scale), ATTN_TC_KV, st)
-            if rc != 2:                     # 2 = shape outside the tcgen05 kernel's envelope -> mma.sync kernel
+            if rc != 2:                     # 2 = shape outside the wgmma kernel's envelope -> mma.sync kernel
                 check(rc, "attn_prefill_tc")
                 _count()
                 return out
@@ -331,7 +329,7 @@ def paged_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tenso
 
 
 def gemm_batched(a: torch.Tensor, w: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
-    """out[:, b, :] = a[:, b, :] @ w[b].T for every batch entry b, on the tcgen05 GEMM's batched mode
+    """out[:, b, :] = a[:, b, :] @ w[b].T for every batch entry b, on the wgmma GEMM's batched mode
     (csrc/gemm/gemm_bf16.cu): a [T, B, K] and out [T, B, N] may be strided views (last dim contiguous) — the operand
     is read through a 3-D TMA map and the result written in place, no transposing copies; w [B, N, K] contiguous.
     MLA weight absorption (per-head q_nope·W_UK and out_lat·W_UV) runs on this instead of a cuBLAS bmm."""

@@ -1,4 +1,4 @@
-"""MoE front-ends: routing kernels + grouped tcgen05 expert GEMMs (csrc/moe/, csrc/gemm/).
+"""MoE front-ends: routing kernels + grouped wgmma expert GEMMs (csrc/moe/, csrc/gemm/).
 
 fused_experts pipeline (reference: gllm/layers/moe/fused_moe_triton/fused_moe.py:768-972):
     align+gather (expert-sorted 128-row tiles) -> grouped GEMM1 with SiLU-gate epilogue

@@ -72,8 +72,7 @@ MAX_BLOCKS = 256   # kMaxBlocks in csrc/comm/tp_fused.cu (128-row blocks per gat
 # SMALL_T: row capacity of the decode-sized all-reduce buffers; forwards with <= small_threshold(tp) tokens run on
 # replicated rows + the one-kernel all-reduce⊕add⊕norm instead of the token-sharded GEMM⊕RS / AG⊕GEMM dataflow (see
 # begin_forward; sweep with benchmarks/tp_small_t_sweep.py). GLLM_TP_SMALL_T=<n> sets both; GLLM_TP_SMALL_T=auto
-# keeps the 64-row buffers and scales the threshold with the LL variant's incoming traffic, (tp-1)*T rows
-# (measured on 8xB200: a 64-token LL step costs 1.8x the 128-token sharded step at TP8, profiles/tp_scaling_r2.md).
+# keeps the 64-row buffers and scales the threshold with the LL variant's incoming traffic, (tp-1)*T rows.
 _SMALL_T_ENV = os.environ.get("GLLM_TP_SMALL_T", "64")
 SMALL_T = 64 if _SMALL_T_ENV == "auto" else int(_SMALL_T_ENV)
 
@@ -194,8 +193,8 @@ class FusedTPComm(TPComm):
     def begin_forward(self, num_tokens: int):
         assert num_tokens <= self.max_tokens
         # Tiny decode batches are latency bound: the swap-AB weight-streaming GEMMs + one NCCL
-        # all-reduce beat the sharded dataflow there (measured on 2xB200: 4.6 ms vs 7.0 ms per step at
-        # batch 16), so such forwards run the baseline strategy; everything else runs fused.
+        # all-reduce beat the sharded dataflow there, so such forwards run the baseline strategy; everything
+        # else runs fused.
         tp = self.tp_size
         # (a forward in which some rank would own no rows of the token-sharded layout stays on the replicated form)
         self.small = num_tokens <= small_threshold(tp) or \

@@ -60,7 +60,7 @@ def dtype_bytes(dtype: torch.dtype) -> int:
 
 
 def device_capability(index: int = 0) -> Optional[int]:
-    """Compute capability as major*10 + minor (100 on B200), None without a CUDA device."""
+    """Compute capability as major*10 + minor (90 on H100), None without a CUDA device."""
     if not torch.cuda.is_available():
         return None
     major, minor = torch.cuda.get_device_capability(index)

@@ -1,5 +1,5 @@
 #!/usr/bin/env bash
-# Build the sm_100a kernel library in-tree and install the package in editable mode.
+# Build the sm_90a kernel library in-tree and install the package in editable mode.
 #   ./install.sh            nvcc build + pip install -e . (no dependency resolution: use requirements.txt for that)
 #   ./install.sh --deps     also install requirements.txt first
 set -euo pipefail

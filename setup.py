@@ -1,6 +1,6 @@
 """Packaging for gllm_b200.
 
-`pip install -e .` (or `pip install .`) compiles the sm_100a kernel library with nvcc through
+`pip install -e .` (or `pip install .`) compiles the sm_90a kernel library with nvcc through
 `gllm_b200.build` — one shared object, no torch C++ headers — and ships it as package data.
 
 Environment:

@@ -1,4 +1,4 @@
-"""sm_100a kernels vs the PyTorch fp32 oracle (runs on the B200 box: `pytest -m gpu`)."""
+"""sm_90a kernels vs the PyTorch fp32 oracle (runs on an H100: `pytest -m gpu`)."""
 import math
 import os
 

@@ -1,5 +1,5 @@
-"""Address arithmetic of the tcgen05 prefill attention kernel (csrc/attn/prefill_attention_tc.cu), checked on the
-CPU against the canonical UMMA shared-memory layouts (CuTe `mma_traits_sm100.hpp`: SW128 K-major
+"""Address arithmetic of the wgmma prefill attention kernel (csrc/attn/prefill_attention_tc.cu), checked on the
+CPU against the canonical wgmma shared-memory layouts (CuTe `mma_traits_sm90_gmma.hpp`: SW128 K-major
 `((8,m),(T,2)):((8T,SBO),(1,T))`, SW128 MN-major `((T,8,m),(8,k)):((1,T,LBO),(8T,SBO))`, T = 8 bf16 per 16 bytes)
 and the 128-byte TMA swizzle. The K-major half of this model is what the GPU-validated GEMM relies on; the test's
 purpose is to catch slips in slab strides, LBO / SBO / K-advance and the hand-written swizzled stores before any
@@ -76,7 +76,8 @@ def test_kv_tiles_assembled_by_tma_match_both_operand_forms(D, KV, page):
 
 @pytest.mark.parametrize("cols", [64, 128])
 def test_hand_swizzled_q_and_p_stores_form_a_kmajor_operand(cols):
-    """Q (cols = D) and P (cols = KV) are written by the softmax threads, 16 bytes at a time, with `a_tile_off`."""
+    """Q (cols = D) is written by the MMA warpgroups, 16 bytes at a time, with `a_tile_off`; the same layout with
+    cols = KV is the K-major form of any 128-row operand tile."""
     rng = np.random.default_rng(1)
     A = rng.integers(1, 60000, size=(128, cols)).astype(np.int64)
     smem = np.zeros(128 * cols, dtype=np.int64)

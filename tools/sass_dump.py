@@ -1,4 +1,4 @@
-"""Commit-able SASS listings of the hot sm_100a kernels (runs without a GPU):
+"""Commit-able SASS listings of the hot sm_90a kernels (runs without a GPU):
 
     python tools/sass_dump.py            # writes profiles/sass/<kernel>.sass
 
@@ -41,7 +41,7 @@ def main():
                 lines.append(f"/*{m.group(1)}*/  {m.group(2).strip()}")
         fn = re.sub(r"[^A-Za-z0-9_]+", "_", hit[0]).strip("_") + ".sass"
         with open(os.path.join(OUT, fn), "w") as f:
-            f.write(f"// {name}\n// {len(lines)} instructions; cuobjdump -sass gllm_b200/_C/libgllm_b200.so (sm_100a)\n")
+            f.write(f"// {name}\n// {len(lines)} instructions; cuobjdump -sass gllm_b200/_C/libgllm_b200.so (sm_90a)\n")
             f.write("\n".join(lines) + "\n")
         done.append((hit[0], len(lines)))
     for k, n in done:
