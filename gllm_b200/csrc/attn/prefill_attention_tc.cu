@@ -306,6 +306,9 @@ GLLM_EXPORT int gllm_attn_prefill_tc(const void* q, int64_t q_ts, void* out, con
                                      int max_blocks, int Hq, int Hkv, int D, int page_size, float scale, int kv_tile,
                                      void* stream) {
   if (num_seqs <= 0 || max_q_len <= 0) return 0;
+  // a page larger than the requested KV tile: stream it as one 128-key tile (the mma.sync kernel, whose tile is 64
+  // keys, cannot take such pages)
+  if (page_size == 128 && kv_tile == 64) kv_tile = 128;
   if ((D != 64 && D != 128) || (kv_tile != 64 && kv_tile != 128) || page_size < 8 || kv_tile % page_size != 0 ||
       Hq % Hkv != 0)
     return 2;

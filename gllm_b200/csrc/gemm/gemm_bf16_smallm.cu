@@ -297,8 +297,10 @@ GLLM_EXPORT int gllm_gemm_smallm(const void* A, int64_t lda, const void* W, int6
                                  int M, int N, int K, const void* bias, int silu, int force_split, void* ws,
                                  int64_t ws_floats, void* counters, void* stream) {
   if (M <= 0 || N <= 0) return 0;
-  if (M > 256 || (K % 8) != 0 || (lda % 8) != 0 || (ldw % 8) != 0) {
-    fprintf(stderr, "[gllm_b200] gemm_smallm: unsupported shape M=%d K=%d\n", M, K);
+  // N and ldc as in gllm_gemm_bf16: the split-K reduction stores 4 bf16 (8 bytes) at C + m * ldc + 4 j
+  if (M > 256 || (K % 8) != 0 || (N % 8) != 0 || (lda % 8) != 0 || (ldw % 8) != 0 || (ldc % 8) != 0) {
+    fprintf(stderr, "[gllm_b200] gemm_smallm: unsupported shape M=%d N=%d K=%d (N, K and leading dims must be "
+            "multiples of 8)\n", M, N, K);
     return 1;
   }
   SmallMParams p;

@@ -53,6 +53,7 @@ def _declare(lib):
     P, I, L, F, U = c_void_p, c_int, c_int64, c_float, c_uint32
     sig("gllm_gemm_bf16", [P, L, P, L, P, L, I, I, I, P, I, I, POINTER(GemmComm), P, L, P, I, P])
     sig("gllm_gemm_bf16_tiles_covering", [I, I, I, I, I, I, I, L, I])
+    sig("gllm_gemm_tune", [I, I])
     sig("gllm_gemm_bf16_batched", [P, L, L, P, P, L, L, I, I, I, I, P])
     sig("gllm_gemm_smallm", [P, L, P, L, P, L, I, I, I, P, I, I, P, L, P, P])
     sig("gllm_rmsnorm", [P, P, P, P, P, I, I, L, F, P])

@@ -15,7 +15,13 @@ from test_kernels_gpu import _make_paged        # the GPU test's paged-input bui
 ROWS = 128
 
 
-def emulate_prefill_tc(q, kc, vc, bt, seq_lens, q_start, hq, hkv, d, page, scale, kv_tile, seq_offset=0):
+def emulate_prefill_tc(q, kc, vc, bt, seq_lens, q_start, hq, hkv, d, page, scale, kv_tile, seq_offset=0,
+                       mutation=None):
+    """`mutation` injects one known slip, for showing that a comparator rejects it (tests/test_wgmma_edges_cpu.py):
+    'horizon+1'  query tile 0 of every sequence sees one key past its causal horizon,
+    'no_alpha'   O is not rescaled when a row max moves,
+    'hbase+1'    the head base of every row block is one group too high (wrapping into the next KV head's heads)."""
+    assert mutation in (None, "horizon+1", "no_alpha", "hbase+1"), mutation
     t = q.shape[0]
     out = torch.zeros(t, hq, d)
     qf = q.view(t, hq, d).float()
@@ -37,19 +43,20 @@ def emulate_prefill_tc(q, kc, vc, bt, seq_lens, q_start, hq, hkv, d, page, scale
             qt = n_qtiles - 1 - bx
             tok_base = qt * toks_per_tile
             last_tok = min(tok_base + toks_per_tile, q_len) - 1
-            kv_end = ctx_len + last_tok + 1
+            leak = 1 if mutation == "horizon+1" and qt == 0 else 0
+            kv_end = ctx_len + last_tok + 1 + leak
             n_tiles = (kv_end + kv_tile - 1) // kv_tile
             last_page = (seq_len - 1) // page
             for bz in range(hkv * (g_all // gp)):                           # blockIdx.z
                 kvh = bz // (g_all // gp)
-                hbase = kvh * g_all + (bz % (g_all // gp)) * gp
+                hbase = kvh * g_all + (bz % (g_all // gp) + (mutation == "hbase+1")) * gp
                 rows = torch.arange(ROWS)
                 tok = tok_base + rows // gp
-                head = hbase + rows % gp
+                head = (hbase + rows % gp) % hq
                 row_ok = tok < q_len
                 qrows = torch.zeros(ROWS, d)
                 qrows[row_ok] = qf[q_begin + tok[row_ok], head[row_ok]]
-                lim = ctx_len + tok
+                lim = ctx_len + tok + leak
                 m_run = torch.full((ROWS,), -math.inf)
                 l_run = torch.zeros(ROWS)
                 o = torch.zeros(ROWS, d)
@@ -64,7 +71,7 @@ def emulate_prefill_tc(q, kc, vc, bt, seq_lens, q_start, hq, hkv, d, page, scale
                     s = qrows @ kt.t()                                       # S = Q K^T (fp32 accumulate)
                     key0 = tile * kv_tile
                     keys = key0 + torch.arange(kv_tile)
-                    need_mask = key0 + kv_tile - 1 > ctx_len + tok_base
+                    need_mask = key0 + kv_tile - 1 > ctx_len + tok_base + leak
                     vis = keys.view(1, -1) <= lim.view(-1, 1) if need_mask else torch.ones(ROWS, kv_tile, dtype=torch.bool)
                     mx = torch.where(vis, s, torch.tensor(-math.inf)).max(dim=1).values
                     m_new = torch.maximum(m_run, mx * scale_log2)
@@ -74,7 +81,7 @@ def emulate_prefill_tc(q, kc, vc, bt, seq_lens, q_start, hq, hkv, d, page, scale
                     p = torch.exp2(s * scale_log2 - m_use.view(-1, 1))
                     p = torch.where(vis, p, torch.zeros(()))
                     l_run = l_run * alpha + p.sum(dim=1)
-                    if tile > 0:
+                    if tile > 0 and mutation != "no_alpha":
                         o = o * alpha.view(-1, 1)       # (the kernel skips this when every alpha of the warp is 1)
                     o = o + p.bfloat16().float() @ vt                        # P is rounded to bf16 for the MMA
                 inv = torch.where(l_run > 0, 1.0 / l_run, torch.zeros(()))

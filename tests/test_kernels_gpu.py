@@ -190,7 +190,7 @@ def test_attn_decode(hq, hkv, d, splits):
 @pytest.mark.parametrize("hq,hkv,d", [(32, 8, 128), (8, 8, 128), (28, 4, 128), (16, 2, 64)])
 def test_attn_prefill_and_mixed(hq, hkv, d, monkeypatch):
     from gllm_b200.ops import sm100
-    monkeypatch.setattr(sm100, "ATTN_TC", False)     # the mma.sync kernel (fallback for shapes outside the tcgen05 one)
+    monkeypatch.setattr(sm100, "ATTN_TC", False)     # the mma.sync kernel (fallback for shapes outside the wgmma one)
     # decode seqs first, then prefill chunks (some with prefix/chunk context)
     seq_lens = [7, 130, 40, 300, 129, 64, 1024]
     q_lens = [1, 1, 40, 100, 129, 3, 513]
@@ -207,7 +207,7 @@ def test_attn_prefill_and_mixed(hq, hkv, d, monkeypatch):
 @pytest.mark.parametrize("kv_tile", [128, 64])
 @pytest.mark.parametrize("hq,hkv,d", [(32, 8, 128), (8, 8, 128), (28, 4, 128), (16, 2, 64)])
 def test_prefill_attention_tc(hq, hkv, d, kv_tile, monkeypatch):
-    """tcgen05 / TMEM prefill kernel vs the fp32 oracle: ragged chunks, prefix context, page-boundary cases."""
+    """wgmma prefill kernel vs the fp32 oracle: ragged chunks, prefix context, page-boundary cases."""
     from gllm_b200.ops import sm100
     monkeypatch.setattr(sm100, "ATTN_TC", True)
     monkeypatch.setattr(sm100, "ATTN_TC_KV", kv_tile)
@@ -271,7 +271,7 @@ def test_sampler_distribution():
 @pytest.mark.parametrize("t", [1, 64, 300])
 @pytest.mark.parametrize("b,n,k", [(16, 512, 128), (16, 128, 512), (3, 256, 192)])
 def test_gemm_batched_strided_views(t, b, n, k):
-    """Batched mode of the tcgen05 GEMM (MLA weight absorption, K13): strided [T, B, K] operand through a 3-D TMA
+    """Batched mode of the wgmma GEMM (MLA weight absorption, K13): strided [T, B, K] operand through a 3-D TMA
     map, result written into a strided [T, B, N] view, vs an fp32 einsum."""
     from gllm_b200.ops import sm100
     torch.manual_seed(t + n)
