@@ -453,6 +453,160 @@ vp_final_kernel(const float* __restrict__ gathered, int tp, int B, int C, int V_
   if (threadIdx.x == 0) out_tokens[row] = tok;
 }
 
+// ------------------------------------------------------------------------------------------------------------------
+// Token log-probabilities of the raw model distribution: log_softmax of the fp32 logits over the real vocabulary,
+// taken before repetition penalty, temperature, top-k and top-p. Vocab-parallel like the sampler above: the [E, V]
+// logits are never gathered. Every TP rank reduces its shard of each requesting row to a record of W = 2N + 3 floats
+//   [0, N)   the shard's N largest raw logits, unordered (-inf where the shard has fewer than N real columns)
+//   [N, 2N)  their token ids bit-cast to float (kLpNoToken where the shard has fewer than N real columns)
+//   2N       shard max m        2N + 1   sum exp(x - m) over the shard
+//   2N + 2   raw logit of the row's sampled token if this shard holds it, -inf otherwise
+// the ranks all-gather the records (tp = 1 on one GPU) and logprobs_final_kernel forms the global log-sum-exp and
+// merges the tp x N candidates to the global top N, ordered by logit, ties to the lower token id (block_argmax's rule).
+// ------------------------------------------------------------------------------------------------------------------
+static constexpr int kMaxLogprobs = 20;
+static constexpr int kLpNoToken = 0x7fffffff;
+
+// One CTA per requesting row. Passes over the row (L2-resident after the LM head): 2 when N == 0 (max, sum exp),
+// 7 when N > 0 (max, sum exp, the 4 radix-select passes for the N-th largest key, one compaction pass).
+template <typename T>
+__global__ void __launch_bounds__(kSampleThreads)
+logprobs_shard_kernel(const T* __restrict__ logits, int64_t ld, int V, int N, const int32_t* __restrict__ rows,
+                      const int32_t* __restrict__ tokens, float* __restrict__ out, int vocab_offset) {
+  __shared__ BlockScratch S;
+  __shared__ int s_cnt, s_eq;
+  const int row = rows != nullptr ? rows[blockIdx.x] : static_cast<int>(blockIdx.x);
+  float* o = out + static_cast<size_t>(blockIdx.x) * (2 * N + 3);
+  GlobalRow<T> R;   // penalty 1, temperature 1: the raw logits
+  R.lr = logits + static_cast<size_t>(row) * ld;
+  R.seen_row = nullptr;
+  R.pen = 1.0f;
+  R.inv_temp = 1.0f;
+  R.vocab_offset = vocab_offset;
+  for (int i = threadIdx.x; i < N; i += blockDim.x) {
+    o[i] = -INFINITY;
+    o[N + i] = __int_as_float(kLpNoToken);
+  }
+  if (threadIdx.x == 0) {
+    s_cnt = 0;
+    s_eq = 0;
+    const int local = tokens[row] - vocab_offset;
+    o[2 * N + 2] = (local >= 0 && local < V) ? R.val(local) : -INFINITY;
+  }
+  if (V <= 0) {   // a shard made of padding only
+    if (threadIdx.x == 0) { o[2 * N] = -INFINITY; o[2 * N + 1] = 0.f; }
+    return;
+  }
+  float vmax = -INFINITY;
+  for (int i = threadIdx.x; i < V; i += blockDim.x) vmax = fmaxf(vmax, R.val(i));
+  const float m = block_max(vmax, S);
+  float z = 0.f;
+  if (m > -INFINITY)
+    for (int i = threadIdx.x; i < V; i += blockDim.x) z += __expf(R.val(i) - m);
+  z = block_sumf(z, S);
+  if (threadIdx.x == 0) { o[2 * N] = m; o[2 * N + 1] = z; }
+  const int k = N < V ? N : V;
+  if (k <= 0) return;
+  // the k largest logits of the shard: radix-select the k-th largest key, then compact
+  radix_select(R, V, 0, 0u, k, 0.f, m, S);
+  const uint32_t thr = S.sel_prefix;
+  const int eq_take = S.sel_k_left;                                // elements with key == thr among the k largest
+  const int eq_all = static_cast<int>(S.hist_cnt[thr & 0xffu]);    // elements with key == thr (last radix pass)
+  __syncthreads();
+  if (eq_take >= eq_all) {
+    // no tie is cut at the k-th place: every key >= thr is taken, in any order
+    for (int i = threadIdx.x; i < V; i += blockDim.x) {
+      const float x = R.val(i);
+      if (f2key(x) >= thr) {
+        const int pos = atomicAdd(&s_cnt, 1);
+        o[pos] = x;
+        o[N + pos] = __int_as_float(i + vocab_offset);
+      }
+    }
+    return;
+  }
+  // a tie is cut at the k-th place: the lowest token ids win, so the equal keys are ranked in index order, one
+  // blockDim-wide chunk at a time (ballot + per-warp prefix counts)
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
+  for (int base = 0; base < V; base += blockDim.x) {
+    const int i = base + threadIdx.x;
+    const float x = i < V ? R.val(i) : -INFINITY;
+    const uint32_t key = i < V ? f2key(x) : 0u;
+    if (i < V && key > thr) {
+      const int pos = atomicAdd(&s_cnt, 1);
+      o[pos] = x;
+      o[N + pos] = __int_as_float(i + vocab_offset);
+    }
+    const bool eq = i < V && key == thr;
+    const unsigned bal = __ballot_sync(0xffffffffu, eq);
+    if (lane == 0) S.ired[warp] = __popc(bal);
+    __syncthreads();
+    int before = s_eq + __popc(bal & ((1u << lane) - 1u));
+    for (int w = 0; w < warp; ++w) before += S.ired[w];
+    if (eq && before < eq_take) {
+      const int pos = atomicAdd(&s_cnt, 1);
+      o[pos] = x;
+      o[N + pos] = __int_as_float(i + vocab_offset);
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      int tot = 0;
+      for (int w = 0; w < nwarps; ++w) tot += S.ired[w];
+      s_eq += tot;
+    }
+    __syncthreads();
+  }
+}
+
+// One CTA per requesting row; `gathered` [tp, E, 2N+3] = every rank's shard records. Writes [E, 1 + 2N] fp32:
+// the sampled token's log-prob, then N x (token id bit-cast to float, log-prob) ordered by logit, ties to the lower
+// token id. Slots beyond the real vocabulary hold token id -1 and log-prob -inf.
+__global__ void __launch_bounds__(256)
+logprobs_final_kernel(const float* __restrict__ gathered, int tp, int E, int N, float* __restrict__ out) {
+  extern __shared__ float cand[];   // [tp * N] logits, then [tp * N] token ids
+  const int row = blockIdx.x;
+  const int W = 2 * N + 3;
+  const size_t rank_stride = static_cast<size_t>(E) * W;
+  const float* rec = gathered + static_cast<size_t>(row) * W;
+  float gm = -INFINITY, chosen = -INFINITY;
+  for (int r = 0; r < tp; ++r) {
+    gm = fmaxf(gm, rec[r * rank_stride + 2 * N]);
+    chosen = fmaxf(chosen, rec[r * rank_stride + 2 * N + 2]);   // -inf on every rank but the token's owner
+  }
+  float gz = 0.f;
+  for (int r = 0; r < tp; ++r) {
+    const float* st = rec + r * rank_stride + 2 * N;
+    if (st[1] > 0.f) gz += st[1] * __expf(st[0] - gm);
+  }
+  const float lse = gm + __logf(gz);
+  float* o = out + static_cast<size_t>(row) * (1 + 2 * N);
+  if (threadIdx.x == 0) o[0] = chosen - lse;
+  const int n = tp * N;
+  int* cand_tok = reinterpret_cast<int*>(cand + n);
+  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+    const int r = i / N, c = i - r * N;
+    cand[i] = rec[r * rank_stride + c];
+    cand_tok[i] = __float_as_int(rec[r * rank_stride + N + c]);
+  }
+  __syncthreads();
+  // rank of candidate i = number of candidates ahead of it in (logit desc, token asc, slot asc) order: a permutation
+  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+    const float v = cand[i];
+    const int t = cand_tok[i];
+    int rank = 0;
+    for (int j = 0; j < n; ++j) {
+      const float vj = cand[j];
+      const int tj = cand_tok[j];
+      rank += (vj > v) || (vj == v && (tj < t || (tj == t && j < i)));
+    }
+    if (rank < N) {
+      const bool real = t != kLpNoToken;
+      o[1 + 2 * rank] = __int_as_float(real ? t : -1);
+      o[2 + 2 * rank] = real ? v - lse : -INFINITY;
+    }
+  }
+}
+
 // set bit `token` of row `row` in the seen-token bitmask: one thread per (row, token) pair
 __global__ void mark_seen_kernel(uint32_t* seen, int seen_words, const int32_t* rows, const int32_t* tokens, int n) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -527,6 +681,35 @@ GLLM_EXPORT int gllm_vp_final(const void* gathered, int tp, int B, int C, int V_
       reinterpret_cast<const float*>(gathered), tp, B, C, V_full, reinterpret_cast<const int32_t*>(top_k),
       reinterpret_cast<const float*>(top_p), seed, reinterpret_cast<const int64_t*>(step_ptr),
       reinterpret_cast<int32_t*>(out_tokens));
+  CUDA_CHECK_RET(cudaGetLastError());
+  return 0;
+}
+
+// Log-probabilities, stage 1: `out` [E, 2N+3] fp32, one record per requesting row (see logprobs_shard_kernel).
+// rows: int32 [E] logits row of each requesting row (null: row i); tokens: int32 sampled token per logits row;
+// V: real vocabulary columns of this shard; vocab_offset: token id of its column 0.
+GLLM_EXPORT int gllm_logprobs_shard(const void* logits, int dtype, int64_t ld, int E, int V, int N, const void* rows,
+                                    const void* tokens, void* out, int vocab_offset, void* stream) {
+  if (N < 0 || N > kMaxLogprobs) return 2;
+  if (E <= 0) return 0;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+#define LP_SHARD(T_)                                                                                               \
+  logprobs_shard_kernel<T_><<<E, kSampleThreads, 0, st>>>(                                                         \
+      reinterpret_cast<const T_*>(logits), ld, V, N, reinterpret_cast<const int32_t*>(rows),                       \
+      reinterpret_cast<const int32_t*>(tokens), reinterpret_cast<float*>(out), vocab_offset)
+  if (dtype == 0) LP_SHARD(__nv_bfloat16); else LP_SHARD(float);
+#undef LP_SHARD
+  CUDA_CHECK_RET(cudaGetLastError());
+  return 0;
+}
+
+// Log-probabilities, stage 2: `gathered` [tp, E, 2N+3] = every rank's stage-1 records -> `out` [E, 1 + 2N] fp32.
+GLLM_EXPORT int gllm_logprobs_final(const void* gathered, int tp, int E, int N, void* out, void* stream) {
+  if (N < 0 || N > kMaxLogprobs || tp <= 0) return 2;
+  if (E <= 0) return 0;
+  const size_t smem = static_cast<size_t>(2) * tp * N * sizeof(float);
+  logprobs_final_kernel<<<E, 256, smem, reinterpret_cast<cudaStream_t>(stream)>>>(
+      reinterpret_cast<const float*>(gathered), tp, E, N, reinterpret_cast<float*>(out));
   CUDA_CHECK_RET(cudaGetLastError());
   return 0;
 }

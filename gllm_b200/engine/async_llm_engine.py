@@ -48,10 +48,23 @@ TPOT_BUCKETS = (0.002, 0.004, 0.006, 0.008, 0.01, 0.015, 0.02, 0.03, 0.04, 0.05,
 E2E_BUCKETS = (0.1, 0.25, 0.5, 1.0, 2.5, 5.0, 10.0, 20.0, 40.0, 60.0, 120.0, 300.0)
 
 
+class Delta(str):
+    """A text delta of a stream that asked for log-probs: `logprobs` lists the entries (token, log-prob,
+    [(token, log-prob), ...]) of the tokens whose text this delta releases (the text may be empty)."""
+    logprobs: list = []
+
+
 class AsyncStream:
-    def __init__(self, raw_request=None, stop=None):
+    def __init__(self, raw_request=None, stop=None, logprobs: bool = False):
         self.stop = [x for x in ([stop] if isinstance(stop, str) else list(stop or [])) if x]
         self._held = ""
+        # log-probs: [text end offset (None until the token's text is put), entry] not delivered yet; an entry leaves
+        # with the delta that releases the last character of its token's text
+        self._lp: Optional[list] = [] if logprobs else None
+        self._text_total = 0     # characters put so far (held ones included)
+        self._released = 0       # characters delivered
+        self.lp_count = 0        # generated tokens whose entry was added
+        self.logprobs_out: list = []   # entries drained by LLM.collect
         self.stop_hit = False
         self._queue: asyncio.Queue = asyncio.Queue()
         self._finished = False
@@ -70,15 +83,20 @@ class AsyncStream:
         finish_reason "stop" and `stop_hit` tells the engine to abort the request."""
         if self._finished:
             return
+        if self._lp is not None:          # the text of the tokens added since the last put ends here
+            self._text_total += len(item)
+            for rec in self._lp:
+                if rec[0] is None:
+                    rec[0] = self._text_total
         if not self.stop:
-            self._queue.put_nowait(item)
+            self._out(item)
             return
         buf = self._held + item
         cut = min((i for i in (buf.find(s) for s in self.stop) if i >= 0), default=-1)
         if cut >= 0:
             self._held = ""
-            if cut:
-                self._queue.put_nowait(buf[:cut])
+            if cut or self._lp:
+                self._out(buf[:cut], everything=True)   # the latest token completed the stop string
             self.stop_hit = True
             self.finish("stop")
             return
@@ -89,14 +107,40 @@ class AsyncStream:
                     hold = k
                     break
         if len(buf) > hold:
-            self._queue.put_nowait(buf[:len(buf) - hold])
+            self._out(buf[:len(buf) - hold])
+        elif self._lp:
+            self._out("")
         self._held = buf[len(buf) - hold:] if hold else ""
+
+    def add_logprobs(self, entries: list):
+        """Entries of tokens whose text the next `put` carries (or a later one, while it is held back)."""
+        if self._lp is not None and not self._finished:
+            self._lp.extend([None, e] for e in entries)
+
+    @property
+    def want_logprobs(self) -> bool:
+        return self._lp is not None
+
+    def _out(self, text: str, everything: bool = False):
+        if self._lp is None:
+            self._queue.put_nowait(text)
+            return
+        self._released += len(text)
+        done = [r for r in self._lp if everything or (r[0] is not None and r[0] <= self._released)]
+        if done:
+            self._lp = [r for r in self._lp if not (everything or (r[0] is not None and r[0] <= self._released))]
+        if text or done:
+            d = Delta(text)
+            d.logprobs = [r[1] for r in done]
+            self._queue.put_nowait(d)
 
     def finish(self, reason: str = "stop"):
         if not self._finished:
             if self._held:                     # generation ended while a possible stop prefix was held back
-                self._queue.put_nowait(self._held)
+                self._out(self._held, everything=True)
                 self._held = ""
+            elif self._lp:                     # entries whose text never came (held U+FFFD tail, empty token text)
+                self._out("", everything=True)
             self.finish_reason = reason
             self._queue.put_nowait(StopAsyncIteration())
             self._finished = True
@@ -137,10 +181,12 @@ class AsyncLLM(LLM):
 
     async def add_requests_async(self, raw_request, token_ids: List[int], output_len=None, ignore_eos=False,
                                  temperature=None, top_p=None, top_k=None, repetition_penalty=None,
-                                 mm_contents=None, stop=None) -> AsyncStream:
+                                 mm_contents=None, stop=None, logprobs=None) -> AsyncStream:
+        """`logprobs`: None, or N in [0, 20] — every text delta of the stream is then a `Delta` carrying the
+        log-prob entries of the tokens whose text it releases (see `LLM.generate`)."""
         seq = self.allocate_seq(token_ids, output_len, ignore_eos, temperature, top_p, top_k, repetition_penalty,
-                                mm_contents)
-        stream = AsyncStream(raw_request, stop)
+                                mm_contents, logprobs)
+        stream = AsyncStream(raw_request, stop, logprobs=logprobs is not None)
         stream.prompt_tokens = len(token_ids)
         stream.seq_id = seq.seq_id
         self.async_streams[seq.seq_id] = stream
@@ -168,7 +214,10 @@ class AsyncLLM(LLM):
         text = ""
         while True:
             try:
-                text += await asyncio.wait_for(stream.__anext__(), timeout=0.5)
+                item = await asyncio.wait_for(stream.__anext__(), timeout=0.5)
+                text += item
+                if isinstance(item, Delta):
+                    stream.logprobs_out.extend(item.logprobs)
             except StopAsyncIteration:
                 return text
             except asyncio.TimeoutError:
@@ -197,7 +246,9 @@ class AsyncLLM(LLM):
                 self.metrics["ttft_count"] += 1
                 self.hist["ttft"].observe(st.first_token_time - st.created)
             st.completion_tokens = seq.num_output_tokens
-            if self.tokenizer is not None:
+            if st.want_logprobs:
+                self._deliver_with_logprobs(seq, st)
+            elif self.tokenizer is not None:
                 delta = seq.detokenize_inc(self.tokenizer)
                 if delta:
                     st.put(delta)
@@ -208,6 +259,28 @@ class AsyncLLM(LLM):
                 st.aborted = True
                 self.abort([seq.seq_id])
         self._pending_tokens = []
+        self._finish_streams()
+
+    def _deliver_with_logprobs(self, seq, st: AsyncStream):
+        """Token by token, so that each log-prob entry leaves with the delta that releases its token's text."""
+        end, lps = seq.known_len, seq.output_logprobs
+        while st.lp_count < len(lps) and not st.finished:
+            j = seq.prompt_len + st.lp_count
+            if j >= end:
+                break
+            chosen, top = lps[st.lp_count]
+            st.add_logprobs([(seq.token_ids[j], chosen, top)])
+            st.lp_count += 1
+            if self.tokenizer is not None:
+                before = seq.cur_length
+                delta = seq.detokenize_inc(self.tokenizer, j + 1)
+                if seq.cur_length != before:
+                    st.put(delta)
+            else:
+                st.put(f"{seq.token_ids[j]} ")
+                seq.cur_length = j + 1
+
+    def _finish_streams(self):
         for seq in self.finished:
             st = self.async_streams.pop(seq.seq_id, None)
             if st is not None:

@@ -4,7 +4,7 @@ Channels (all PUSH/PULL, HWM 0):
     front-end -> driver      requests / aborts / control commands          (pickled IPCPackage)
     driver    -> front-end   sampled tokens / freed ids                    (pickled IPCPackage)
     driver    -> every peer  one scheduled micro-batch per message         (header + raw arrays)
-    output rank -> driver    sampled tokens of a finished micro-batch
+    output rank -> driver    sampled tokens (and log-probs) of a finished micro-batch
 
 Differences from the reference: a micro-batch travels as flat numpy buffers (`BatchArrays`),
 not as pickled `Sequence` objects that every rank re-expands in Python; sends are issued from the
@@ -33,6 +33,7 @@ class IPCPackage:
     abort_ids: list = field(default_factory=list)
     act_schedule_ids: list = field(default_factory=list)  # driver -> front-end
     next_tokens: list = field(default_factory=list)
+    next_logprobs: Optional[list] = None   # aligned with next_tokens when some request asked for log-probs
     free_ids: list = field(default_factory=list)
     control_cmd: Optional[tuple] = None
     stats: Optional[dict] = None
@@ -207,8 +208,9 @@ class Comm:
         return "batch", self._decode_batch(buf[1:])
 
     # output rank -> driver -----------------------------------------------------------------------
-    def send_tokens(self, batch_id: int, tokens: List[int]):
-        self.tok_out.send(pickle.dumps((batch_id, tokens), protocol=pickle.HIGHEST_PROTOCOL))
+    def send_tokens(self, batch_id: int, tokens: List[int], logprobs: Optional[list] = None):
+        """`logprobs`: None, or one entry per token (see StepResult.logprobs_list)."""
+        self.tok_out.send(pickle.dumps((batch_id, tokens, logprobs), protocol=pickle.HIGHEST_PROTOCOL))
 
     def recv_tokens(self):
         out = []

@@ -29,6 +29,8 @@ from gllm_b200.id_allocator import IDAllocator
 from gllm_b200.model_loader import ModelLoader
 from gllm_b200.parallel import state as ps
 from gllm_b200.sequence import Sequence
+
+MAX_LOGPROBS = 20   # most likely tokens reported per generated token (csrc/sample/sampler.cu: kMaxLogprobs)
 from gllm_b200.utils.logging import logger
 
 
@@ -207,9 +209,12 @@ class LLM:
         return True
 
     def allocate_seq(self, token_ids: List[int], output_len=None, ignore_eos=False, temperature=None, top_p=None,
-                     top_k=None, repetition_penalty=None, mm_contents=None) -> Sequence:
+                     top_k=None, repetition_penalty=None, mm_contents=None, logprobs=None) -> Sequence:
         """Defaults: temperature/top_p/repetition_penalty from generation_config, top_k = 1
-        (greedy) unless given (reference: gllm/llm_engine.py:305-337)."""
+        (greedy) unless given (reference: gllm/llm_engine.py:305-337). `logprobs`: None (no log-probs) or the number
+        N in [0, MAX_LOGPROBS] of most likely tokens to report next to every generated token's log-prob."""
+        if logprobs is not None and not 0 <= int(logprobs) <= MAX_LOGPROBS:
+            raise ValueError(f"logprobs must be in [0, {MAX_LOGPROBS}]")
         if len(token_ids) == 0:
             raise ValueError("empty prompt: there is no position to sample the first token from")
         vocab = self.loader.config.get("vocab_size")
@@ -222,7 +227,7 @@ class LLM:
                        self.default_top_p if top_p is None else top_p,
                        1 if top_k is None else top_k,
                        self.default_repetition_penalty if repetition_penalty is None else repetition_penalty,
-                       mm_contents)
+                       mm_contents, -1 if logprobs is None else int(logprobs))
         if output_len is None:
             seq.output_len = min(4096, self.model_max_length - len(token_ids))
         if mm_contents:
@@ -278,12 +283,15 @@ class LLM:
     def _apply(self, pkg: IPCPackage, on_token=None):
         now = time.time()
         inproc = self.worker is not None
-        for sid, tok in zip(pkg.act_schedule_ids, pkg.next_tokens):
+        lps = pkg.next_logprobs
+        for i, (sid, tok) in enumerate(zip(pkg.act_schedule_ids, pkg.next_tokens)):
             seq = self.running_maps.get(sid)
             if seq is None:
                 continue
             if not inproc:
                 seq.append(tok)  # in-proc: the scheduler already appended to the shared object
+            if lps is not None and lps[i] is not None:
+                seq.output_logprobs.append(lps[i])   # only here: the scheduler never touches output_logprobs
             if seq.first_token_time == 0.0:
                 seq.first_token_time = now
             if on_token is not None:
@@ -317,10 +325,13 @@ class LLM:
     def generate(self, prompts: Optional[List[str]] = None, tokens: Optional[List[List[int]]] = None,
                  output_lens: Optional[List[int]] = None, temperature=None, top_p=None, top_k=None,
                  repetition_penalty=None, ignore_eos: bool = False, progress: bool = False,
-                 mm_contents: Optional[List[Optional[dict]]] = None) -> List[Sequence]:
+                 mm_contents: Optional[List[Optional[dict]]] = None, logprobs=None) -> List[Sequence]:
         """Batch generation; returns the finished `Sequence`s in request order with `.prompt`,
         `.output`, `.token_ids` (reference: gllm/llm_engine.py:343-378). `mm_contents[i]` (VL models) is
-        the processor output of request i: pixel_values / image_grid_thw [/ pixel_values_videos ...]."""
+        the processor output of request i: pixel_values / image_grid_thw [/ pixel_values_videos ...].
+        `logprobs` (None or N in [0, 20], one value or one per request): every generated token gets an entry
+        (its log-prob, [(token, log-prob) of the N most likely tokens]) in `.output_logprobs`, under the raw model
+        distribution (log_softmax of the logits, before penalty / temperature / top-k / top-p)."""
         if self.worker is not None and self.worker.rank != 0:
             return self._serve_until_stop()
         if tokens is None:
@@ -337,7 +348,7 @@ class LLM:
                 return v[i] if isinstance(v, (list, tuple)) else v
             seqs.append(self.allocate_seq(toks, ol, ignore_eos, pick(temperature), pick(top_p), pick(top_k),
                                           pick(repetition_penalty),
-                                          mm_contents[i] if mm_contents is not None else None))
+                                          mm_contents[i] if mm_contents is not None else None, pick(logprobs)))
         self.add_requests(seqs)
         base = len(self.finished)
         bar = None

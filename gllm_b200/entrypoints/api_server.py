@@ -45,6 +45,52 @@ def _validate_sampling(request):
     return None
 
 
+MAX_LOGPROBS = 20
+
+
+def _validate_logprobs(request, chat: bool):
+    if chat:
+        n = request.top_logprobs or 0
+        if not 0 <= n <= MAX_LOGPROBS:
+            return f"top_logprobs must be in [0, {MAX_LOGPROBS}]"
+        if n > 0 and not request.logprobs:
+            return "top_logprobs requires logprobs to be true"
+        return None
+    if request.logprobs is not None and not 0 <= request.logprobs <= MAX_LOGPROBS:
+        return f"logprobs must be in [0, {MAX_LOGPROBS}]"
+    return None
+
+
+def _token_str(tok: int) -> str:
+    return llm.tokenizer.decode([tok]) if llm.tokenizer is not None else f"token_id:{tok}"
+
+
+def _lp_num(lp: float) -> float:
+    return max(lp, -9999.0)      # JSON has no -inf (a token whose logit is -inf)
+
+
+def _chat_logprobs(entries):
+    """OpenAI chat shape: {"content": [{token, logprob, bytes, top_logprobs: [{token, logprob, bytes}]}]}."""
+    def one(tok, lp):
+        s = _token_str(tok)
+        return {"token": s, "logprob": _lp_num(lp), "bytes": list(s.encode("utf-8"))}
+    return {"content": [dict(one(tok, lp), top_logprobs=[one(t, v) for t, v in top]) for tok, lp, top in entries]}
+
+
+def _completion_logprobs(entries, offset: int = 0):
+    """Legacy completions shape {tokens, token_logprobs, top_logprobs: [{token: logprob}], text_offset}; `offset` is
+    the text offset of the first entry. Returns (logprobs, offset after the last entry)."""
+    out = {"tokens": [], "token_logprobs": [], "top_logprobs": [], "text_offset": []}
+    for tok, lp, top in entries:
+        s = _token_str(tok)
+        out["tokens"].append(s)
+        out["token_logprobs"].append(_lp_num(lp))
+        out["top_logprobs"].append({_token_str(t): _lp_num(v) for t, v in top})
+        out["text_offset"].append(offset)
+        offset += len(s)
+    return out, offset
+
+
 def _validate(token_ids, output_len, vocab_size=None):
     """-> error message or None. An empty prompt or a token id outside the vocabulary would take the whole engine
     down (there is no row to sample from / the embedding lookup faults), so they are refused at the door."""
@@ -71,6 +117,8 @@ async def chat_completion_generator(stream, request) -> ChatCompletionResponse:
     text = await llm.collect(stream)
     choice = ChatCompletionResponseChoice(index=0, message=ChatMessage(role="assistant", content=text),
                                           finish_reason=stream.finish_reason)
+    if stream.want_logprobs:
+        choice.logprobs = _chat_logprobs(stream.logprobs_out)
     return ChatCompletionResponse(choices=[choice], usage=_usage(stream), model=request.model)
 
 
@@ -83,6 +131,8 @@ async def chat_completion_stream_generator(stream, request):
             first = False
             chunk = ChatCompletionStreamResponse(
                 choices=[ChatCompletionResponseStreamChoice(index=0, delta=dm)], model=request.model)
+            if stream.want_logprobs:
+                chunk.choices[0].logprobs = _chat_logprobs(delta.logprobs)
             if rid is None:
                 rid = chunk.id
             chunk.id = rid
@@ -102,15 +152,20 @@ async def chat_completion_stream_generator(stream, request):
 async def completion_generator(stream, request) -> CompletionResponse:
     text = await llm.collect(stream)
     choice = CompletionResponseChoice(index=0, text=text, finish_reason=stream.finish_reason)
+    if stream.want_logprobs:
+        choice.logprobs = _completion_logprobs(stream.logprobs_out)[0]
     return CompletionResponse(choices=[choice], model=request.model, usage=_usage(stream))
 
 
 async def completion_stream_generator(stream, request):
     rid = None
+    offset = 0
     try:
         async for delta in stream:
             chunk = CompletionStreamResponse(choices=[CompletionResponseStreamChoice(index=0, text=delta)],
                                              model=request.model)
+            if stream.want_logprobs:
+                chunk.choices[0].logprobs, offset = _completion_logprobs(delta.logprobs, offset)
             if rid is None:
                 rid = chunk.id
             chunk.id = rid
@@ -200,15 +255,16 @@ def build_app(engine):
                 token_ids = await _in_thread(llm.encode, None, True, request.messages)
         except Exception as e:  # noqa: BLE001
             return _error(f"cannot encode messages: {e}")
-        bad = _validate_sampling(request) or _validate(token_ids, request.output_len(),
-                                                       llm.loader.config.get("vocab_size"))
+        bad = _validate_sampling(request) or _validate_logprobs(request, chat=True) or \
+            _validate(token_ids, request.output_len(), llm.loader.config.get("vocab_size"))
         if bad:
             return _error(bad)
         if llm.failed:
             return _error(f"engine is down: {llm.failed}", HTTPStatus.INTERNAL_SERVER_ERROR)
         stream = await llm.add_requests_async(raw_request, token_ids, request.output_len(), request.ignore_eos,
                                               request.temperature, request.top_p, request.top_k,
-                                              request.repetition_penalty, mm_contents, stop=request.stop)
+                                              request.repetition_penalty, mm_contents, stop=request.stop,
+                                              logprobs=(request.top_logprobs or 0) if request.logprobs else None)
         if request.stream:
             return StreamingResponse(chat_completion_stream_generator(stream, request),
                                      media_type="text/event-stream")
@@ -220,15 +276,16 @@ def build_app(engine):
             token_ids = await _in_thread(_encode_prompt, request.prompt)
         except Exception as e:  # noqa: BLE001
             return _error(f"cannot encode prompt: {e}")
-        bad = _validate_sampling(request) or _validate(token_ids, request.max_tokens,
-                                                       llm.loader.config.get("vocab_size"))
+        bad = _validate_sampling(request) or _validate_logprobs(request, chat=False) or \
+            _validate(token_ids, request.max_tokens, llm.loader.config.get("vocab_size"))
         if bad:
             return _error(bad)
         if llm.failed:
             return _error(f"engine is down: {llm.failed}", HTTPStatus.INTERNAL_SERVER_ERROR)
         stream = await llm.add_requests_async(raw_request, token_ids, request.max_tokens, request.ignore_eos,
                                               request.temperature, request.top_p, request.top_k,
-                                              request.repetition_penalty, stop=request.stop)
+                                              request.repetition_penalty, stop=request.stop,
+                                              logprobs=request.logprobs)
         if request.stream:
             return StreamingResponse(completion_stream_generator(stream, request), media_type="text/event-stream")
         return JSONResponse(content=(await completion_generator(stream, request)).model_dump())

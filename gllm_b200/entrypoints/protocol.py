@@ -3,6 +3,15 @@
 Written against the public OpenAI API shape; field coverage follows what the reference accepts
 (gllm/entrypoints/protocol.py:165-716) plus a filled `usage`. Unknown request fields are ignored
 rather than rejected so stock OpenAI clients work unchanged.
+
+Log-probabilities (chat `logprobs` + `top_logprobs`, completions `logprobs: N`) are those of the raw model
+distribution: log_softmax in fp32 of the logits the LM head produced, over the real vocabulary, before repetition
+penalty, temperature, top-k and top-p. So they do not depend on the sampling parameters, and the sampled token's
+log-prob is reported under that distribution even when it was drawn with a temperature or a filter. Every generated
+token gets its log-prob and the N most likely tokens (0 <= N <= 20), ordered by logit, ties to the lower token id; for
+a greedy request the first of them is the sampled token. Prompt tokens get none (`echo` is ignored). Token strings are
+`tokenizer.decode([id])` (`bytes`: its UTF-8 encoding), or "token_id:<id>" without a tokenizer. A log-prob of -inf is
+reported as -9999.0. Out-of-range `top_logprobs` / `logprobs`, or `top_logprobs > 0` without `logprobs`, is a 400.
 """
 from __future__ import annotations
 

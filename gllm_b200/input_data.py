@@ -58,6 +58,8 @@ class BatchArrays:
     # lookahead (async scheduling): row i takes its input token from element feed_src[i] of the PREVIOUS step's
     # device-side sampler output instead of `tokens[i]` (which holds a placeholder)
     feed_src: Optional[np.ndarray] = None
+    # int32 [E]: top alternatives whose log-probs each emitting row wants (-1: none); None when no row asks
+    logprobs_n: Optional[np.ndarray] = None
     emit_ids: Optional[list] = None  # driver-local: sequence id per EMITTING entry (order of the sampler output)
     seq_ids: Optional[list] = None  # driver-local: sequence id per row (incremental decode batches); not sent
     pt_gens: Optional[list] = None  # driver-local: Sequence.pt_gen per row when the block table rows were written
@@ -71,7 +73,7 @@ class BatchArrays:
         (16-byte aligned sections) so a batch costs two zmq frames per peer instead of one per array."""
         names = ["tokens", "positions", "slot_mapping", "block_table", "seq_lens", "query_start_loc",
                  "logits_idx", "emit_seq", "temperature", "top_k", "top_p", "rep_penalty", "state_slot"]
-        opt = ["seen_rows", "seen_tokens", "clear_slots", "feed_src"]
+        opt = ["seen_rows", "seen_tokens", "clear_slots", "feed_src", "logprobs_n"]
         hdr = {"scalars": (self.num_decode_seqs, self.num_seqs, self.num_tokens, self.max_q_len,
                            self.max_seq_len, self.all_greedy, self.need_penalty, self.batch_id),
                "arrays": [], "mm": self.mm}
@@ -159,11 +161,15 @@ def _build_decode_fast(entries, page_size: int, batch_id: int, prev: "BatchArray
     slots = bt[rows, blk] * page_size + starts % page_size
     seq_lens = starts + 1
     feed = perm.astype(np.int32) if (tokens < 0).any() else None   # lookahead rows: token still on the device
+    lp_n = prev.logprobs_n[perm] if prev.logprobs_n is not None else None
+    if lp_n is not None and not (lp_n >= 0).any():
+        lp_n = None        # the rows that asked have finished: the batch is what it would be without the feature
     return BatchArrays(feed_src=feed,
         tokens=tokens, positions=starts, slot_mapping=slots.astype(np.int32), block_table=bt, seq_lens=seq_lens,
         query_start_loc=prev.query_start_loc[:b + 1], logits_idx=prev.logits_idx[:b], emit_seq=prev.emit_seq[:b],
         temperature=prev.temperature[perm], top_k=prev.top_k[perm], top_p=prev.top_p[perm],
-        rep_penalty=prev.rep_penalty[perm], state_slot=prev.state_slot[perm], num_decode_seqs=b, num_seqs=b, num_tokens=b, max_q_len=1,
+        rep_penalty=prev.rep_penalty[perm], state_slot=prev.state_slot[perm],
+        logprobs_n=lp_n, num_decode_seqs=b, num_seqs=b, num_tokens=b, max_q_len=1,
         max_seq_len=int(seq_lens.max()), all_greedy=prev.all_greedy, need_penalty=False, batch_id=batch_id,
         seq_ids=ids, emit_ids=ids, pt_gens=gens)
 
@@ -198,6 +204,7 @@ def build_batch(entries, page_size: int, vocab_size: int, batch_id: int = 0, mro
     emit_seq, logits_idx = [], []
     temperature, top_k, top_p, rep_pen, state_slot = [], [], [], [], []
     seen_rows, seen_tokens, clear_slots = [], [], []
+    logprobs_n, want_logprobs = [], False
     all_greedy, need_penalty = True, False
     for i, e in enumerate(entries):
         seq = e.seq
@@ -232,6 +239,9 @@ def build_batch(entries, page_size: int, vocab_size: int, batch_id: int = 0, mro
             top_p.append(seq.top_p)
             rep_pen.append(seq.repetition_penalty)
             state_slot.append(seq.slot)
+            logprobs_n.append(seq.logprobs)
+            if seq.logprobs >= 0:
+                want_logprobs = True
             if top_k[-1] != 1:
                 all_greedy = False
             if seq.repetition_penalty != 1.0:
@@ -261,6 +271,7 @@ def build_batch(entries, page_size: int, vocab_size: int, batch_id: int = 0, mro
         seen_rows=np.concatenate(seen_rows) if seen_rows else None,
         seen_tokens=np.concatenate(seen_tokens) if seen_tokens else None,
         clear_slots=np.asarray(clear_slots, dtype=np.int32) if clear_slots else None, batch_id=batch_id, mm=mm,
+        logprobs_n=np.asarray(logprobs_n, dtype=np.int32) if want_logprobs else None,
         seq_ids=[e.seq.seq_id for e in entries] if n_dec == b else None,
         pt_gens=[e.seq.pt_gen for e in entries] if n_dec == b else None,
         emit_ids=[entries[i].seq.seq_id for i in emit_seq])

@@ -37,6 +37,11 @@ class StepResult:
     hidden: Optional[torch.Tensor] = None
     residual: Optional[torch.Tensor] = None
     num_emit: int = 0
+    # log-probabilities (only when some emitting row asked): fp32 [E_lp, 1 + 2N] for the asking rows in emit order,
+    # its pinned copy (same event as tokens_host) and the int32 [E] request (-1: none) per emitting row
+    logprobs: Optional[torch.Tensor] = None
+    logprobs_host: Optional[torch.Tensor] = None
+    logprobs_n: Optional[np.ndarray] = None
 
     def tokens_list(self) -> List[int]:
         if self.tokens is None:
@@ -45,6 +50,27 @@ class StepResult:
             self.event.synchronize()
             return self.tokens_host[: self.num_emit].tolist()
         return self.tokens[: self.num_emit].tolist()
+
+    def logprobs_list(self) -> Optional[list]:
+        """None when no row asked; else per emitting row None or (sampled token's log-prob, [(token, log-prob), ...]
+        with the row's N most likely tokens, largest first)."""
+        if self.logprobs_n is None:
+            return None
+        lp = self.logprobs
+        if self.event is not None:
+            self.event.synchronize()
+            lp = self.logprobs_host[: lp.numel()].view(lp.shape)
+        vals = lp.cpu().numpy()
+        ids = vals.view(np.int32)
+        out, j = [], 0
+        for n in self.logprobs_n[: self.num_emit].tolist():
+            if n < 0:
+                out.append(None)
+                continue
+            top = [(int(ids[j, 1 + 2 * i]), float(vals[j, 2 + 2 * i])) for i in range(n) if ids[j, 1 + 2 * i] >= 0]
+            out.append((float(vals[j, 0]), top))
+            j += 1
+        return out
 
 
 class ModelRunner:
@@ -125,6 +151,7 @@ class ModelRunner:
                                   for _ in range(2)]
             self._host_flip = 0
             self.tokens_host = self._tokens_host2[0]
+            self._lp_host2 = None        # pinned log-prob result buffers, allocated on the first request that asks
             self.step_counter = torch.zeros(1, dtype=torch.int64, device=self.device)
         logger.info("model loaded in %.1fs", time.time() - t0)
         self.profile_run()
@@ -317,7 +344,8 @@ class ModelRunner:
             full = self.tpc.gather_logits(logits, self.spec.vocab_size) if self.vp_sample else logits
             self.logit_log.append((list(batch.emit_ids or []), full[:e, : self.spec.vocab_size].float().cpu()))
         if self.vp_sample and batch.all_greedy and not batch.need_penalty:
-            return self._finish_sample(self._vp_greedy(logits), e)
+            toks = self._vp_greedy(logits)
+            return self._finish_sample(toks, e, self._logprobs(batch, logits, toks, vocab_parallel=True))
         if self.vp_sample and not self.vp_candidates:
             logits = self.tpc.gather_logits(logits, self.spec.vocab_size)   # GLLM_VP_SAMPLE=greedy: A/B switch
         seen = None
@@ -340,9 +368,47 @@ class ModelRunner:
         if not batch.all_greedy:
             self.step_counter += 1
         if self.vp_sample and self.vp_candidates:
-            return self._finish_sample(self._vp_sample(logits, seen), e)
+            toks = self._vp_sample(logits, seen)
+            return self._finish_sample(toks, e, self._logprobs(batch, logits, toks, vocab_parallel=True))
         toks = Fn.sample(logits, inp, seen, seed=self.cfg.seed, step=self.step_counter)
-        return self._finish_sample(toks, e)
+        return self._finish_sample(toks, e, self._logprobs(batch, logits, toks, vocab_parallel=False))
+
+    def _logprobs(self, batch: BatchArrays, logits: torch.Tensor, toks: torch.Tensor,
+                  vocab_parallel: bool) -> Optional[torch.Tensor]:
+        """Log-probabilities of the raw model distribution for the emitting rows that asked (csrc/sample/sampler.cu:
+        logprobs_shard_kernel / logprobs_final_kernel), after the tokens are chosen. `vocab_parallel`: `logits` is this
+        rank's vocab shard — every TP rank reduces its shard to [E_lp, 2N+3] records and the ranks all-gather them
+        (every rank decides from the batch alone, so all of them join the collective). None when no row asked: then
+        the step launches, exchanges and copies nothing more than without this feature."""
+        lpn = batch.logprobs_n
+        if lpn is None:
+            return None
+        want = np.nonzero(lpn >= 0)[0].astype(np.int32)
+        if want.size == 0:
+            return None
+        n = int(lpn[want].max())
+        rows = torch.from_numpy(want).to(logits.device)
+        toks = toks.to(torch.int32).contiguous()
+        v_full = self.spec.vocab_size
+        tp, off, valid = 1, 0, v_full
+        if vocab_parallel:
+            st = ps.get_state()
+            per = logits.shape[1]
+            tp, off = st.tp_size, st.tp_rank * per
+            valid = max(0, min(per, v_full - off))   # the last rank's shard ends with padding columns
+        if logits.is_cuda:
+            from gllm_b200.ops import sm100 as ops
+        else:
+            from gllm_b200.ops import ref as ops
+        rec = ops.logprobs_shard(logits, valid, n, toks, rows, vocab_offset=off)
+        if tp > 1:
+            import torch.distributed as dist
+            allr = torch.empty(tp, *rec.shape, dtype=torch.float32, device=rec.device)
+            dist.all_gather_into_tensor(allr.view(tp * rec.shape[0], rec.shape[1]), rec, group=ps.get_state().tp_group)
+        else:
+            allr = rec.unsqueeze(0)
+        self.stats["logprob_rows"] = self.stats.get("logprob_rows", 0) + len(want)
+        return ops.logprobs_final(allr, n)
 
     VP_CANDIDATES = 256   # per rank and row; top_k <= this is exact (csrc/sample/sampler.cu)
 
@@ -418,17 +484,30 @@ class ModelRunner:
         best = allp[:, :, 0].argmax(dim=0, keepdim=True)
         return allp[:, :, 1].gather(0, best)[0].to(torch.int32)
 
-    def _finish_sample(self, toks: torch.Tensor, e: int) -> StepResult:
+    def _finish_sample(self, toks: torch.Tensor, e: int, logprobs: Optional[torch.Tensor] = None) -> StepResult:
         self.tokens_out[:e].copy_(toks)
         # (CPU: no async D2H copy — snapshot the values, a lookahead step may overwrite tokens_out before the
         # scheduler reads them)
         res = StepResult(tokens=self.tokens_out if self.device.type == "cuda" else self.tokens_out[:e].clone(),
                          num_emit=e)
+        if logprobs is not None:
+            res.logprobs, res.logprobs_n = logprobs, self.input_data.batch.logprobs_n[:e]
         if self.device.type == "cuda":
             self._host_flip ^= 1
             self.tokens_host = self._tokens_host2[self._host_flip]
             self.tokens_host[:e].copy_(self.tokens_out[:e], non_blocking=True)
             self.stats["d2h_bytes"] += 4 * e
+            if logprobs is not None:
+                # two pinned buffers, flipped with tokens_host: a lookahead step's copy may land before the host has
+                # read this one
+                if self._lp_host2 is None:
+                    from gllm_b200.ops.sm100 import MAX_LOGPROBS
+                    size = max(self.max_running_seqs, 1) * (1 + 2 * MAX_LOGPROBS)
+                    self._lp_host2 = [torch.zeros(size, dtype=torch.float32, pin_memory=True) for _ in range(2)]
+                host = self._lp_host2[self._host_flip]
+                host[: logprobs.numel()].copy_(logprobs.view(-1), non_blocking=True)
+                res.logprobs_host = host
+                self.stats["d2h_bytes"] += 4 * logprobs.numel()
             ev = torch.cuda.Event()
             ev.record()
             res.tokens_host, res.event = self.tokens_host, ev

@@ -71,6 +71,8 @@ def _declare(lib):
     sig("gllm_mark_seen", [P, I, P, P, I, P])
     sig("gllm_vp_candidates", [P, I, L, P, I, I, I, I, P, P, P, P, P, I, P, c_uint64, P, I, P])
     sig("gllm_vp_final", [P, I, I, I, I, P, P, c_uint64, P, P, P])
+    sig("gllm_logprobs_shard", [P, I, L, I, I, I, P, P, P, I, P])
+    sig("gllm_logprobs_final", [P, I, I, I, P, P])
     sig("gllm_moe_topk_softmax", [P, L, P, P, I, I, I, I, P])
     sig("gllm_moe_grouped_topk", [P, L, P, P, P, I, I, I, I, I, I, I, F, P])
     sig("gllm_moe_align_gather", [P, P, I, I, I, P, P, I, P, P, L, P, I, P, P])

@@ -356,6 +356,63 @@ def vp_final(gathered: torch.Tensor, c: int, v_full: int, top_k=None, top_p=None
     return out
 
 
+LP_NO_TOKEN = 0x7fffffff   # token id of an empty candidate slot in a log-prob record
+
+
+def logprobs_shard(logits: torch.Tensor, valid: int, n: int, tokens: torch.Tensor,
+                   rows: Optional[torch.Tensor] = None, vocab_offset: int = 0) -> torch.Tensor:
+    """PyTorch model of csrc/sample/sampler.cu:logprobs_shard_kernel — per requesting row a record [E, 2n+3]: the
+    shard's n largest raw logits (lower token id first on ties), their token ids bit-cast to float, shard max, shard
+    sum-exp, and the raw logit of the sampled token if this shard holds it (-inf otherwise)."""
+    x_all = logits if rows is None else logits[rows.long()]
+    toks = tokens if rows is None else tokens[rows.long()]
+    e = x_all.shape[0]
+    out = torch.full((e, 2 * n + 3), float("-inf"), dtype=torch.float32, device=logits.device)
+    ids = out.view(torch.int32)
+    ids[:, n:2 * n] = LP_NO_TOKEN
+    out[:, 2 * n + 1] = 0.0
+    if valid <= 0 or e == 0:
+        return out
+    x = x_all[:, :valid].float()
+    m = x.max(dim=-1).values
+    finite = m > float("-inf")
+    out[:, 2 * n] = m
+    out[:, 2 * n + 1] = torch.where(finite, torch.exp(x - torch.where(finite, m, 0.0).view(-1, 1)).sum(-1), 0.0)
+    local = toks.long() - vocab_offset
+    mine = (local >= 0) & (local < valid)
+    chosen = x.gather(1, local.clamp(0, valid - 1).view(-1, 1))[:, 0]
+    out[:, 2 * n + 2] = torch.where(mine, chosen, float("-inf"))
+    k = min(n, valid)
+    if k:
+        vals, idx = torch.sort(x, dim=-1, descending=True, stable=True)
+        out[:, :k] = vals[:, :k]
+        ids[:, n:n + k] = (idx[:, :k] + vocab_offset).to(torch.int32)
+    return out
+
+
+def logprobs_final(gathered: torch.Tensor, n: int) -> torch.Tensor:
+    """PyTorch model of logprobs_final_kernel: [tp, E, 2n+3] records -> [E, 1 + 2n] = sampled token's log-prob, then
+    n x (token id bit-cast to float, log-prob) by logit, ties to the lower id; id -1 / -inf past the vocabulary."""
+    tp, e, _ = gathered.shape
+    ms, zs, ch = gathered[:, :, 2 * n], gathered[:, :, 2 * n + 1], gathered[:, :, 2 * n + 2]
+    gm = ms.max(dim=0).values
+    gz = (zs * torch.exp(torch.where(zs > 0, ms - gm.view(1, -1), torch.zeros_like(ms)))).sum(0)
+    lse = gm + torch.log(gz)
+    out = torch.empty(e, 1 + 2 * n, dtype=torch.float32, device=gathered.device)
+    out[:, 0] = ch.max(dim=0).values - lse
+    if n:
+        vals = gathered[:, :, :n].permute(1, 0, 2).reshape(e, tp * n)
+        toks = gathered[:, :, n:2 * n].contiguous().view(torch.int32).permute(1, 0, 2).reshape(e, tp * n)
+        o1 = torch.argsort(toks, dim=1, stable=True)                  # token ascending, then logit descending (stable)
+        vals, toks = vals.gather(1, o1), toks.gather(1, o1)
+        o2 = torch.argsort(vals, dim=1, descending=True, stable=True)[:, :n]
+        vals, toks = vals.gather(1, o2), toks.gather(1, o2)
+        real = toks != LP_NO_TOKEN
+        out.view(torch.int32)[:, 1::2] = torch.where(real, toks, torch.full_like(toks, -1))
+        out[:, 2::2] = torch.where(real, vals - lse.view(-1, 1), torch.full_like(vals, float("-inf")))
+    return out
+
+
 # ----------------------------------------------------------------------------------------------
 # MoE
 # ----------------------------------------------------------------------------------------------

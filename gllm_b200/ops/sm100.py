@@ -408,6 +408,42 @@ def vp_final(gathered: torch.Tensor, c: int, v_full: int, top_k=None, top_p=None
     return out
 
 
+MAX_LOGPROBS = 20
+
+
+def logprobs_shard(logits: torch.Tensor, valid: int, n: int, tokens: torch.Tensor,
+                   rows: Optional[torch.Tensor] = None, vocab_offset: int = 0) -> torch.Tensor:
+    """Log-probabilities, stage 1 (csrc/sample/sampler.cu:logprobs_shard_kernel): per requesting row a record
+    [E, 2n+3] fp32 — this shard's n largest raw logits and their token ids, the shard's (max, sum exp) and the raw logit
+    of the sampled token if this shard holds it. `logits` [B, >= valid] bf16/fp32 (this rank's vocab shard, or the full
+    row); `valid` real vocabulary columns; `tokens` int32 [B] sampled tokens; `rows` int32 [E] logits row of each
+    requesting row (None: all B rows)."""
+    assert logits.dim() == 2 and logits.stride(1) == 1 and logits.dtype in (_BF16, torch.float32)
+    assert 0 <= n <= MAX_LOGPROBS and tokens.dtype == torch.int32 and tokens.is_contiguous()
+    assert rows is None or (rows.dtype == torch.int32 and rows.is_contiguous())
+    e = logits.shape[0] if rows is None else rows.numel()
+    out = torch.empty(e, 2 * n + 3, dtype=torch.float32, device=logits.device)
+    L = _lib.load()
+    rc = L.gllm_logprobs_shard(_p(logits), 0 if logits.dtype == _BF16 else 1, logits.stride(0), e, valid, n, _p(rows),
+                               _p(tokens), _p(out), vocab_offset, stream_ptr())
+    check(rc, "logprobs_shard")
+    _count()
+    return out
+
+
+def logprobs_final(gathered: torch.Tensor, n: int) -> torch.Tensor:
+    """Log-probabilities, stage 2: `gathered` [tp, E, 2n+3] (every rank's stage-1 records) -> [E, 1 + 2n] fp32: the
+    sampled token's log-prob, then n x (token id bit-cast to float, log-prob), largest logit first, ties to the lower
+    id; id -1 / -inf past the real vocabulary."""
+    tp, e, w = gathered.shape
+    assert w == 2 * n + 3 and gathered.is_contiguous() and gathered.dtype == torch.float32
+    out = torch.empty(e, 1 + 2 * n, dtype=torch.float32, device=gathered.device)
+    L = _lib.load()
+    check(L.gllm_logprobs_final(_p(gathered), tp, e, n, _p(out), stream_ptr()), "logprobs_final")
+    _count()
+    return out
+
+
 def mark_seen(seen_bits: torch.Tensor, rows: torch.Tensor, tokens: torch.Tensor):
     assert rows.dtype == torch.int32 and tokens.dtype == torch.int32
     L = _lib.load()

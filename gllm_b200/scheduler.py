@@ -84,6 +84,9 @@ class SchedulerOutput:
     act_schedule_ids: List[int] = field(default_factory=list)
     next_tokens: List[int] = field(default_factory=list)
     free_ids: List[int] = field(default_factory=list)
+    # aligned with next_tokens when some row of the batch asked for log-probs (entry None for rows that did not),
+    # None otherwise
+    next_logprobs: Optional[list] = None
 
 
 class Scheduler:
@@ -108,6 +111,7 @@ class Scheduler:
         self.seqs_to_decode: Deque[Sequence] = deque()
         self.batch_running: Deque[List[ScheduledSeq]] = deque()
         self.next_tokens_queue: Deque[List[int]] = deque()
+        self.next_logprobs_queue: Deque[Optional[list]] = deque()   # one entry per next_tokens_queue entry
         self.abort_ids = set()
         self.on_preempt = None      # callback(seq): the owner releases per-sequence device state
         self.num_preempt_seqs = 0
@@ -138,8 +142,10 @@ class Scheduler:
     def add_abort_ids(self, ids):
         self.abort_ids.update(ids)
 
-    def add_next_tokens(self, next_tokens: List[int]):
+    def add_next_tokens(self, next_tokens: List[int], next_logprobs: Optional[list] = None):
+        """`next_logprobs`: None, or one entry per emitting row (None where the row did not ask)."""
         self.next_tokens_queue.append(next_tokens)
+        self.next_logprobs_queue.append(next_logprobs)
 
     def set_log(self, log: bool):
         self.log = log
@@ -161,7 +167,10 @@ class Scheduler:
             return None
         batch = self.batch_running.popleft()
         next_tokens = self.next_tokens_queue.popleft()
+        next_logprobs = self.next_logprobs_queue.popleft()
         out = SchedulerOutput()
+        if next_logprobs is not None:
+            out.next_logprobs = []
         prefix, ps = isinstance(self.mm, PrefixMemoryManager), self.page_size
         k = 0  # next_tokens holds one token per *emitting* entry, in batch order
         for ent in batch:
@@ -198,6 +207,8 @@ class Scheduler:
                 tok = int(next_tokens[k - 1])
                 out.act_schedule_ids.append(seq.seq_id)
                 out.next_tokens.append(tok)
+                if next_logprobs is not None:
+                    out.next_logprobs.append(next_logprobs[k - 1])
                 ahead = seq.pending == ent.start + ent.n   # a lookahead step already follows this one
                 if ahead:
                     seq.token_ids[seq.pending] = tok

@@ -10,11 +10,12 @@ class Sequence:
                  "repetition_penalty", "computed_token_num", "scheduled_token_num", "is_abort",
                  "mm_contents", "page_hashes", "num_cached_tokens", "arrival_time", "first_token_time",
                  "finish_time", "slot", "mrope_delta", "mm_state", "pt_np", "pending", "zombie", "pt_gen", "published",
-                 "slot_fresh")
+                 "slot_fresh", "logprobs", "output_logprobs")
 
     def __init__(self, seq_id: int, token_ids: List[int], finish_tokens: List[int],
                  output_len: Optional[int] = None, ignore_eos: bool = False, temperature: float = 0.6,
-                 top_p: float = 0.9, top_k: int = 10, repetition_penalty: float = 1.0, mm_contents=None):
+                 top_p: float = 0.9, top_k: int = 10, repetition_penalty: float = 1.0, mm_contents=None,
+                 logprobs: int = -1):
         self.seq_id = seq_id
         self.token_ids: List[int] = list(token_ids)
         self.prompt_len = len(self.token_ids)
@@ -30,6 +31,10 @@ class Sequence:
         self.top_p = top_p
         self.top_k = top_k
         self.repetition_penalty = repetition_penalty
+        # log-probabilities: how many top alternatives to report per generated token (-1: none), and one entry
+        # (sampled token's log-prob, [(token, log-prob), ...]) per generated token, filled by the front-end
+        self.logprobs = logprobs
+        self.output_logprobs: list = []
         # computed_token_num : tokens whose KV is computed AND whose batch has returned
         # scheduled_token_num: tokens covered by chunks scheduled so far (returned or in flight);
         #                      with pp_size > 1 several chunks of one prompt can be in flight
@@ -97,9 +102,10 @@ class Sequence:
         """Number of tokens whose values are known on the host (a trailing lookahead placeholder is not)."""
         return len(self.token_ids) - (1 if self.pending >= 0 else 0)
 
-    def detokenize_inc(self, tokenizer) -> str:
-        """Incremental detokenisation; holds back while the tail decodes to U+FFFD."""
-        end = self.known_len
+    def detokenize_inc(self, tokenizer, end: Optional[int] = None) -> str:
+        """Incremental detokenisation of the tokens up to `end` (default: every known token); holds back while the
+        tail decodes to U+FFFD."""
+        end = self.known_len if end is None else end
         if self.cur_length >= end:
             return ""
         prev = tokenizer.decode(self.token_ids[self.cur_length - 1: self.cur_length + 1],
