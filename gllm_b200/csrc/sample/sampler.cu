@@ -10,6 +10,13 @@
 //            the same distribution the reference draws with `probs / Exp(1)` then argmax)
 // Greedy rows (top_k == 1) take a single argmax pass. A vocab-parallel variant returns the
 // per-rank (max, index) pair so TP ranks only exchange B x 2 scalars (SURVEY §2.4 X4).
+//
+// Per-request sampling parameters (OpenAI `frequency_penalty` / `presence_penalty` / `logit_bias` / `seed`):
+//   bias row : a row with one adds bias[slot, token] to the penalised logit before the temperature,
+//              x2 = penalty(x) - f * c_j - p * [c_j > 0] + logit_bias_j. The row is persistent per-slot state kept
+//              by bias_rebuild_kernel (slot (re)assignment) and bias_account_kernel (after every sampled token).
+//   seed     : a seeded row keys its exponential race by (seed, position of the token being produced, token id)
+//              instead of (engine seed + step counter, batch row, token id), so its draw depends on the logits alone.
 #include "../common/host_utils.h"
 #include "../common/ptx.cuh"
 
@@ -46,11 +53,36 @@ template <>
 __device__ __forceinline__ float load_logit<float>(const float* p, int i) { return p[i]; }
 
 // seen: optional [B, ceil(V/32)] bitmask of tokens that already appeared (prompt + output)
-__device__ __forceinline__ float transform(float x, int i, const uint32_t* seen_row, float penalty, float inv_temp) {
+// bias_row: optional full-vocabulary additive row (frequency / presence penalties and logit_bias), indexed by token id
+__device__ __forceinline__ float transform(float x, int i, const uint32_t* seen_row, float penalty,
+                                           const float* bias_row, float inv_temp) {
   if (seen_row != nullptr && penalty != 1.0f) {
     if ((seen_row[i >> 5] >> (i & 31)) & 1u) x = x > 0.f ? x / penalty : x * penalty;
   }
+  if (bias_row != nullptr) x += bias_row[i];
   return x * inv_temp;
+}
+
+// Per-row RNG key of the exponential race: (engine seed + step, batch row) by default; (request seed, position of the
+// token being produced) for a seeded row (seed_pos >= 0).
+__device__ __forceinline__ void race_key(const int64_t* seeds, const int32_t* seed_pos, int row, uint64_t seed,
+                                         uint32_t step, uint64_t& key, uint32_t& krow) {
+  key = seed + step;
+  krow = static_cast<uint32_t>(row);
+  if (seeds != nullptr && seed_pos != nullptr) {
+    const int pos = seed_pos[row];
+    if (pos >= 0) {
+      key = static_cast<uint64_t>(seeds[row]);
+      krow = static_cast<uint32_t>(pos);
+    }
+  }
+}
+
+__device__ __forceinline__ const float* bias_row_of(const float* bias, int64_t bias_ld, const int32_t* bias_slot,
+                                                    int row) {
+  if (bias == nullptr || bias_slot == nullptr) return nullptr;
+  const int s = bias_slot[row];
+  return s >= 0 ? bias + static_cast<size_t>(s) * bias_ld : nullptr;
 }
 
 struct BlockScratch {
@@ -120,10 +152,11 @@ template <typename T>
 struct GlobalRow {
   const T* lr;
   const uint32_t* seen_row;
+  const float* bias_row;
   float pen, inv_temp;
   int vocab_offset;
   __device__ __forceinline__ float val(int i) const {
-    return transform(load_logit<T>(lr, i), i + vocab_offset, seen_row, pen, inv_temp);
+    return transform(load_logit<T>(lr, i), i + vocab_offset, seen_row, pen, bias_row, inv_temp);
   }
   __device__ __forceinline__ int token(int i) const { return i + vocab_offset; }
 };
@@ -245,7 +278,9 @@ sample_kernel(const T* __restrict__ logits, int64_t ld, int V, const float* __re
               const int32_t* __restrict__ top_k, const float* __restrict__ top_p,
               const float* __restrict__ rep_penalty, const uint32_t* __restrict__ seen, int seen_words,
               const int32_t* __restrict__ slot_idx, uint64_t seed, const int64_t* __restrict__ step_ptr, int32_t* __restrict__ out_tokens,
-              float* __restrict__ out_max, int vocab_offset) {
+              float* __restrict__ out_max, int vocab_offset, const float* __restrict__ bias, int64_t bias_ld,
+              const int32_t* __restrict__ bias_slot, const int64_t* __restrict__ seeds,
+              const int32_t* __restrict__ seed_pos) {
   __shared__ BlockScratch S;
   const int row = blockIdx.x;
   const uint32_t* seen_row =
@@ -254,6 +289,7 @@ sample_kernel(const T* __restrict__ logits, int64_t ld, int V, const float* __re
   GlobalRow<T> R;
   R.lr = logits + static_cast<size_t>(row) * ld;
   R.seen_row = seen_row;
+  R.bias_row = bias_row_of(bias, bias_ld, bias_slot, row);
   R.inv_temp = (temp <= 1e-5f) ? 1.0f : 1.0f / temp;
   R.pen = rep_penalty != nullptr ? rep_penalty[row] : 1.0f;
   R.vocab_offset = vocab_offset;
@@ -281,9 +317,12 @@ sample_kernel(const T* __restrict__ logits, int64_t ld, int V, const float* __re
   for (int i = threadIdx.x; i < V; i += blockDim.x) z += __expf(R.val(i) - m);
   const float mass_all = block_sumf(z, S);
   const uint32_t step = step_ptr != nullptr ? static_cast<uint32_t>(*step_ptr) : 0u;
+  uint64_t key;
+  uint32_t krow;
+  race_key(seeds, seed_pos, row, seed, step, key, krow);
   float best;
   int tok;
-  select_and_draw(R, V, k, tp, m, mass_all, seed + step, static_cast<uint32_t>(row), S, best, tok);
+  select_and_draw(R, V, k, tp, m, mass_all, key, krow, S, best, tok);
   if (threadIdx.x == 0) {
     out_tokens[row] = tok;
     if (out_max != nullptr) out_max[row] = best;
@@ -308,7 +347,9 @@ vp_candidates_kernel(const T* __restrict__ logits, int64_t ld, int V, int V_full
                      const float* __restrict__ temperature, const int32_t* __restrict__ top_k,
                      const float* __restrict__ top_p, const float* __restrict__ rep_penalty,
                      const uint32_t* __restrict__ seen, int seen_words, const int32_t* __restrict__ slot_idx,
-                     uint64_t seed, const int64_t* __restrict__ step_ptr, float* __restrict__ out, int vocab_offset) {
+                     uint64_t seed, const int64_t* __restrict__ step_ptr, float* __restrict__ out, int vocab_offset,
+                     const float* __restrict__ bias, int64_t bias_ld, const int32_t* __restrict__ bias_slot,
+                     const int64_t* __restrict__ seeds, const int32_t* __restrict__ seed_pos) {
   __shared__ BlockScratch S;
   __shared__ int s_cnt, s_eq;
   const int row = blockIdx.x;
@@ -320,6 +361,7 @@ vp_candidates_kernel(const T* __restrict__ logits, int64_t ld, int V, int V_full
   GlobalRow<T> R;
   R.lr = logits + static_cast<size_t>(row) * ld;
   R.seen_row = seen_row;
+  R.bias_row = bias_row_of(bias, bias_ld, bias_slot, row);
   R.inv_temp = (temp <= 1e-5f) ? 1.0f : 1.0f / temp;
   R.pen = rep_penalty != nullptr ? rep_penalty[row] : 1.0f;
   R.vocab_offset = vocab_offset;
@@ -352,11 +394,14 @@ vp_candidates_kernel(const T* __restrict__ logits, int64_t ld, int V, int V_full
     // unfiltered row: the exponential race needs no normalisation, run it on the shard (scores are relative to the
     // shard max m: the final kernel shifts them to the global max)
     const uint32_t step = step_ptr != nullptr ? static_cast<uint32_t>(*step_ptr) : 0u;
+    uint64_t key;
+    uint32_t krow;
+    race_key(seeds, seed_pos, row, seed, step, key, krow);
     float best = -INFINITY;
     int besti = 0x7fffffff;
     for (int i = threadIdx.x; i < V; i += blockDim.x) {
       const float x = R.val(i);
-      const float e = rand_exp(seed + step, static_cast<uint32_t>(row), static_cast<uint32_t>(i + vocab_offset));
+      const float e = rand_exp(key, krow, static_cast<uint32_t>(i + vocab_offset));
       const float score = (x - m) - __logf(e);
       if (score > best || (score == best && i + vocab_offset < besti)) { best = score; besti = i + vocab_offset; }
     }
@@ -396,7 +441,8 @@ vp_candidates_kernel(const T* __restrict__ logits, int64_t ld, int V, int V_full
 __global__ void __launch_bounds__(256)
 vp_final_kernel(const float* __restrict__ gathered, int tp, int B, int C, int V_full,
                 const int32_t* __restrict__ top_k, const float* __restrict__ top_p, uint64_t seed,
-                const int64_t* __restrict__ step_ptr, int32_t* __restrict__ out_tokens) {
+                const int64_t* __restrict__ step_ptr, int32_t* __restrict__ out_tokens,
+                const int64_t* __restrict__ seeds, const int32_t* __restrict__ seed_pos) {
   __shared__ BlockScratch S;
   const int row = blockIdx.x;
   const int W = 2 * C + 4;
@@ -448,7 +494,10 @@ vp_final_kernel(const float* __restrict__ gathered, int tp, int B, int C, int V_
     block_argmax(v, t, S);
     tok = t;
   } else {
-    select_and_draw(R, n, k, tpv, gm, gz, seed + step, static_cast<uint32_t>(row), S, best, tok);
+    uint64_t key;
+    uint32_t krow;
+    race_key(seeds, seed_pos, row, seed, step, key, krow);
+    select_and_draw(R, n, k, tpv, gm, gz, key, krow, S, best, tok);
   }
   if (threadIdx.x == 0) out_tokens[row] = tok;
 }
@@ -480,6 +529,7 @@ logprobs_shard_kernel(const T* __restrict__ logits, int64_t ld, int V, int N, co
   GlobalRow<T> R;   // penalty 1, temperature 1: the raw logits
   R.lr = logits + static_cast<size_t>(row) * ld;
   R.seen_row = nullptr;
+  R.bias_row = nullptr;
   R.pen = 1.0f;
   R.inv_temp = 1.0f;
   R.vocab_offset = vocab_offset;
@@ -616,6 +666,67 @@ __global__ void mark_seen_kernel(uint32_t* seen, int seen_words, const int32_t* 
   atomicOr(&seen[static_cast<size_t>(rows[i]) * seen_words + (tok >> 5)], 1u << (tok & 31));
 }
 
+// ------------------------------------------------------------------------------------------------------------------
+// Bias rows of the frequency / presence penalties and logit_bias. Per slot: an fp32 row bias[slot, V] holding
+// -f * c_j - p * [c_j > 0] + logit_bias_j and a bitmask out_seen[slot, ceil(V/32)] of the tokens generated so far
+// (c_j > 0), so the presence term is charged once. Every sampling rank keeps full-vocabulary rows.
+//
+// Ordering invariant: both kernels run on the compute stream, after the forward and the sampler of their step. A
+// lookahead step still in flight when its sequence finishes (a zombie row) therefore completes its accounting on the
+// slot before any later batch can rebuild and reuse that slot: the rebuild is enqueued behind it on the same stream.
+// ------------------------------------------------------------------------------------------------------------------
+
+// One thread per emitting row: charge the token just sampled. Rows without a bias row (bias_slot < 0) do nothing.
+// A slot appears at most once per step (one sequence per slot, one token per sequence), so nothing races.
+__global__ void bias_account_kernel(float* __restrict__ bias, int64_t bias_ld, uint32_t* __restrict__ out_seen,
+                                    int seen_words, const int32_t* __restrict__ bias_slot,
+                                    const int32_t* __restrict__ tokens, const float* __restrict__ freq,
+                                    const float* __restrict__ pres, int E) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= E) return;
+  const int slot = bias_slot[r];
+  const int tok = tokens[r];
+  if (slot < 0 || tok < 0) return;
+  uint32_t* w = out_seen + static_cast<size_t>(slot) * seen_words + (tok >> 5);
+  const uint32_t bit = 1u << (tok & 31);
+  const bool first = (atomicOr(w, bit) & bit) == 0u;
+  float* b = bias + static_cast<size_t>(slot) * bias_ld + tok;
+  *b = *b - (first ? freq[r] + pres[r] : freq[r]);
+}
+
+// One CTA per (re)assigned slot: clear the row, scatter the request's logit_bias, then replay the counts of the output
+// tokens known so far in output order — the same fp32 operations bias_account_kernel performs token by token, so a
+// recomputed sequence gets back bit for bit the row it had. Thread t replays the tokens of the bitmask words w with
+// w % blockDim == t, in order, so every element (and every out_seen word) has exactly one writer.
+__global__ void __launch_bounds__(1024)
+bias_rebuild_kernel(float* __restrict__ bias, int64_t bias_ld, uint32_t* __restrict__ out_seen, int seen_words,
+                    int V, const int32_t* __restrict__ slots, const float* __restrict__ pen,
+                    const int32_t* __restrict__ lb_off, const int32_t* __restrict__ lb_ids,
+                    const float* __restrict__ lb_vals, const int32_t* __restrict__ out_off,
+                    const int32_t* __restrict__ out_toks) {
+  const int r = blockIdx.x;
+  const int slot = slots[r];
+  float* row = bias + static_cast<size_t>(slot) * bias_ld;
+  uint32_t* seen = out_seen + static_cast<size_t>(slot) * seen_words;
+  for (int i = threadIdx.x; i < V; i += blockDim.x) row[i] = 0.f;
+  for (int i = threadIdx.x; i < seen_words; i += blockDim.x) seen[i] = 0u;
+  __syncthreads();
+  for (int i = lb_off[r] + threadIdx.x; i < lb_off[r + 1]; i += blockDim.x) {
+    const int tok = lb_ids[i];
+    if (tok >= 0 && tok < V) row[tok] = lb_vals[i];   // (ids are validated on the host; never write past the row)
+  }
+  __syncthreads();
+  const float f = pen[2 * r], p = pen[2 * r + 1];
+  for (int i = out_off[r]; i < out_off[r + 1]; ++i) {
+    const int tok = out_toks[i];
+    if (tok < 0 || tok >= V || (tok >> 5) % static_cast<int>(blockDim.x) != static_cast<int>(threadIdx.x)) continue;
+    const uint32_t bit = 1u << (tok & 31);
+    const bool first = (seen[tok >> 5] & bit) == 0u;
+    seen[tok >> 5] |= bit;
+    row[tok] = row[tok] - (first ? f + p : f);
+  }
+}
+
 }  // namespace b200
 
 using namespace b200;
@@ -628,7 +739,8 @@ GLLM_EXPORT int gllm_sample(const void* logits, int dtype, int64_t ld, void* out
                             const void* temperature, const void* top_k, const void* top_p,
                             const void* rep_penalty, const void* seen, int seen_words,
                             const void* slot_idx, uint64_t seed,
-                            const void* step_ptr, void* out_max, int vocab_offset, void* stream) {
+                            const void* step_ptr, void* out_max, int vocab_offset, const void* bias, int64_t bias_ld,
+                            const void* bias_slot, const void* seeds, const void* seed_pos, void* stream) {
   if (B <= 0) return 0;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   if (dtype == 0) {
@@ -638,7 +750,9 @@ GLLM_EXPORT int gllm_sample(const void* logits, int dtype, int64_t ld, void* out
         reinterpret_cast<const float*>(rep_penalty), reinterpret_cast<const uint32_t*>(seen), seen_words,
         reinterpret_cast<const int32_t*>(slot_idx), seed,
         reinterpret_cast<const int64_t*>(step_ptr), reinterpret_cast<int32_t*>(out_tokens),
-        reinterpret_cast<float*>(out_max), vocab_offset);
+        reinterpret_cast<float*>(out_max), vocab_offset, reinterpret_cast<const float*>(bias), bias_ld,
+        reinterpret_cast<const int32_t*>(bias_slot), reinterpret_cast<const int64_t*>(seeds),
+        reinterpret_cast<const int32_t*>(seed_pos));
   } else {
     sample_kernel<float><<<B, kSampleThreads, 0, st>>>(
         reinterpret_cast<const float*>(logits), ld, V, reinterpret_cast<const float*>(temperature),
@@ -646,7 +760,9 @@ GLLM_EXPORT int gllm_sample(const void* logits, int dtype, int64_t ld, void* out
         reinterpret_cast<const float*>(rep_penalty), reinterpret_cast<const uint32_t*>(seen), seen_words,
         reinterpret_cast<const int32_t*>(slot_idx), seed,
         reinterpret_cast<const int64_t*>(step_ptr), reinterpret_cast<int32_t*>(out_tokens),
-        reinterpret_cast<float*>(out_max), vocab_offset);
+        reinterpret_cast<float*>(out_max), vocab_offset, reinterpret_cast<const float*>(bias), bias_ld,
+        reinterpret_cast<const int32_t*>(bias_slot), reinterpret_cast<const int64_t*>(seeds),
+        reinterpret_cast<const int32_t*>(seed_pos));
   }
   CUDA_CHECK_RET(cudaGetLastError());
   return 0;
@@ -656,7 +772,9 @@ GLLM_EXPORT int gllm_sample(const void* logits, int dtype, int64_t ld, void* out
 GLLM_EXPORT int gllm_vp_candidates(const void* logits, int dtype, int64_t ld, void* out, int B, int V, int V_full,
                                    int C, const void* temperature, const void* top_k, const void* top_p,
                                    const void* rep_penalty, const void* seen, int seen_words, const void* slot_idx,
-                                   uint64_t seed, const void* step_ptr, int vocab_offset, void* stream) {
+                                   uint64_t seed, const void* step_ptr, int vocab_offset, const void* bias,
+                                   int64_t bias_ld, const void* bias_slot, const void* seeds, const void* seed_pos,
+                                   void* stream) {
   if (B <= 0) return 0;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
 #define VP_CAND(T_)                                                                                                \
@@ -665,7 +783,9 @@ GLLM_EXPORT int gllm_vp_candidates(const void* logits, int dtype, int64_t ld, vo
       reinterpret_cast<const int32_t*>(top_k), reinterpret_cast<const float*>(top_p),                              \
       reinterpret_cast<const float*>(rep_penalty), reinterpret_cast<const uint32_t*>(seen), seen_words,            \
       reinterpret_cast<const int32_t*>(slot_idx), seed, reinterpret_cast<const int64_t*>(step_ptr),                \
-      reinterpret_cast<float*>(out), vocab_offset)
+      reinterpret_cast<float*>(out), vocab_offset, reinterpret_cast<const float*>(bias), bias_ld,              \
+      reinterpret_cast<const int32_t*>(bias_slot), reinterpret_cast<const int64_t*>(seeds),                        \
+      reinterpret_cast<const int32_t*>(seed_pos))
   if (dtype == 0) VP_CAND(__nv_bfloat16); else VP_CAND(float);
 #undef VP_CAND
   CUDA_CHECK_RET(cudaGetLastError());
@@ -675,12 +795,13 @@ GLLM_EXPORT int gllm_vp_candidates(const void* logits, int dtype, int64_t ld, vo
 // Vocab-parallel sampling, stage 2: `gathered` [tp, B, 2C+4] = every rank's stage-1 records.
 GLLM_EXPORT int gllm_vp_final(const void* gathered, int tp, int B, int C, int V_full, const void* top_k,
                               const void* top_p, uint64_t seed, const void* step_ptr, void* out_tokens,
-                              void* stream) {
+                              const void* seeds, const void* seed_pos, void* stream) {
   if (B <= 0) return 0;
   vp_final_kernel<<<B, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       reinterpret_cast<const float*>(gathered), tp, B, C, V_full, reinterpret_cast<const int32_t*>(top_k),
       reinterpret_cast<const float*>(top_p), seed, reinterpret_cast<const int64_t*>(step_ptr),
-      reinterpret_cast<int32_t*>(out_tokens));
+      reinterpret_cast<int32_t*>(out_tokens), reinterpret_cast<const int64_t*>(seeds),
+      reinterpret_cast<const int32_t*>(seed_pos));
   CUDA_CHECK_RET(cudaGetLastError());
   return 0;
 }
@@ -720,6 +841,34 @@ GLLM_EXPORT int gllm_mark_seen(void* seen, int seen_words, const void* rows, con
   mark_seen_kernel<<<(n + 255) / 256, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       reinterpret_cast<uint32_t*>(seen), seen_words, reinterpret_cast<const int32_t*>(rows),
       reinterpret_cast<const int32_t*>(tokens), n);
+  CUDA_CHECK_RET(cudaGetLastError());
+  return 0;
+}
+
+// Bias rows: charge the sampled token of every emitting row that has one (see bias_account_kernel).
+GLLM_EXPORT int gllm_bias_account(void* bias, int64_t bias_ld, void* out_seen, int seen_words, const void* bias_slot,
+                                  const void* tokens, const void* freq, const void* pres, int E, void* stream) {
+  if (E <= 0) return 0;
+  bias_account_kernel<<<(E + 127) / 128, 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      reinterpret_cast<float*>(bias), bias_ld, reinterpret_cast<uint32_t*>(out_seen), seen_words,
+      reinterpret_cast<const int32_t*>(bias_slot), reinterpret_cast<const int32_t*>(tokens),
+      reinterpret_cast<const float*>(freq), reinterpret_cast<const float*>(pres), E);
+  CUDA_CHECK_RET(cudaGetLastError());
+  return 0;
+}
+
+// Bias rows: rebuild R (re)assigned slots (see bias_rebuild_kernel). pen: fp32 [R, 2] (frequency, presence);
+// lb_off / out_off: int32 [R + 1] offsets into lb_ids / lb_vals and out_toks.
+GLLM_EXPORT int gllm_bias_rebuild(void* bias, int64_t bias_ld, void* out_seen, int seen_words, int V, int R,
+                                  const void* slots, const void* pen, const void* lb_off, const void* lb_ids,
+                                  const void* lb_vals, const void* out_off, const void* out_toks, void* stream) {
+  if (R <= 0) return 0;
+  bias_rebuild_kernel<<<R, 1024, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      reinterpret_cast<float*>(bias), bias_ld, reinterpret_cast<uint32_t*>(out_seen), seen_words, V,
+      reinterpret_cast<const int32_t*>(slots), reinterpret_cast<const float*>(pen),
+      reinterpret_cast<const int32_t*>(lb_off), reinterpret_cast<const int32_t*>(lb_ids),
+      reinterpret_cast<const float*>(lb_vals), reinterpret_cast<const int32_t*>(out_off),
+      reinterpret_cast<const int32_t*>(out_toks));
   CUDA_CHECK_RET(cudaGetLastError());
   return 0;
 }

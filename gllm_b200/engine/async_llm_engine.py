@@ -181,11 +181,13 @@ class AsyncLLM(LLM):
 
     async def add_requests_async(self, raw_request, token_ids: List[int], output_len=None, ignore_eos=False,
                                  temperature=None, top_p=None, top_k=None, repetition_penalty=None,
-                                 mm_contents=None, stop=None, logprobs=None) -> AsyncStream:
+                                 mm_contents=None, stop=None, logprobs=None, seed=None, frequency_penalty=None,
+                                 presence_penalty=None, logit_bias=None) -> AsyncStream:
         """`logprobs`: None, or N in [0, 20] — every text delta of the stream is then a `Delta` carrying the
-        log-prob entries of the tokens whose text it releases (see `LLM.generate`)."""
+        log-prob entries of the tokens whose text it releases (see `LLM.generate`). `seed`, `frequency_penalty`,
+        `presence_penalty`, `logit_bias`: see `LLM.allocate_seq` (ValueError when out of range)."""
         seq = self.allocate_seq(token_ids, output_len, ignore_eos, temperature, top_p, top_k, repetition_penalty,
-                                mm_contents, logprobs)
+                                mm_contents, logprobs, seed, frequency_penalty, presence_penalty, logit_bias)
         stream = AsyncStream(raw_request, stop, logprobs=logprobs is not None)
         stream.prompt_tokens = len(token_ids)
         stream.seq_id = seq.seq_id

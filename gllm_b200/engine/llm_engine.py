@@ -31,6 +31,49 @@ from gllm_b200.parallel import state as ps
 from gllm_b200.sequence import Sequence
 
 MAX_LOGPROBS = 20   # most likely tokens reported per generated token (csrc/sample/sampler.cu: kMaxLogprobs)
+# logit_bias entries per request: this engine's own cap (one scatter per entry when the bias row is rebuilt)
+MAX_LOGIT_BIAS = 1024
+
+
+def check_sampling_params(seed=None, frequency_penalty=None, presence_penalty=None, logit_bias=None,
+                          vocab_size=None):
+    """Validate and normalise the OpenAI sampling parameters -> (seed or None, frequency_penalty, presence_penalty,
+    {token id: bias} or None). Raises ValueError: penalties must be finite and in [-2, 2]; logit_bias takes at most
+    MAX_LOGIT_BIAS entries whose keys parse as ints in [0, vocab_size) and whose values are finite and in
+    [-100, 100] (a key given twice, e.g. "7" and "07", keeps the last value); seed must fit a signed 64-bit int."""
+    import math
+    out = []
+    for name, v in (("frequency_penalty", frequency_penalty), ("presence_penalty", presence_penalty)):
+        v = 0.0 if v is None else float(v)
+        if not (math.isfinite(v) and -2.0 <= v <= 2.0):
+            raise ValueError(f"{name} must be a finite number in [-2, 2]")
+        out.append(v)
+    if seed is not None:
+        if isinstance(seed, bool) or int(seed) != seed or not -2 ** 63 <= int(seed) < 2 ** 63:
+            raise ValueError("seed must be an integer that fits in a signed 64-bit int")
+        seed = int(seed)
+    lb = None
+    if logit_bias:
+        if len(logit_bias) > MAX_LOGIT_BIAS:
+            raise ValueError(f"logit_bias takes at most {MAX_LOGIT_BIAS} entries")
+        if vocab_size is None:
+            raise ValueError("logit_bias needs a model with a known vocabulary size")
+        lb = {}
+        for k, v in logit_bias.items():
+            try:
+                tok = int(k)
+            except (TypeError, ValueError):
+                raise ValueError(f"logit_bias key {k!r} is not a token id") from None
+            if not 0 <= tok < vocab_size:
+                raise ValueError(f"logit_bias key {k!r} must be a token id in [0, {vocab_size})")
+            try:
+                val = float(v)
+            except (TypeError, ValueError):
+                raise ValueError(f"logit_bias value for {k!r} is not a number") from None
+            if not (math.isfinite(val) and -100.0 <= val <= 100.0):
+                raise ValueError(f"logit_bias value for {k!r} must be a finite number in [-100, 100]")
+            lb[tok] = val
+    return seed, out[0], out[1], lb
 from gllm_b200.utils.logging import logger
 
 
@@ -209,12 +252,17 @@ class LLM:
         return True
 
     def allocate_seq(self, token_ids: List[int], output_len=None, ignore_eos=False, temperature=None, top_p=None,
-                     top_k=None, repetition_penalty=None, mm_contents=None, logprobs=None) -> Sequence:
+                     top_k=None, repetition_penalty=None, mm_contents=None, logprobs=None, seed=None,
+                     frequency_penalty=None, presence_penalty=None, logit_bias=None) -> Sequence:
         """Defaults: temperature/top_p/repetition_penalty from generation_config, top_k = 1
         (greedy) unless given (reference: gllm/llm_engine.py:305-337). `logprobs`: None (no log-probs) or the number
-        N in [0, MAX_LOGPROBS] of most likely tokens to report next to every generated token's log-prob."""
+        N in [0, MAX_LOGPROBS] of most likely tokens to report next to every generated token's log-prob.
+        `seed`, `frequency_penalty`, `presence_penalty`, `logit_bias`: OpenAI semantics, validated by
+        `check_sampling_params` (see entrypoints/protocol.py for the formula)."""
         if logprobs is not None and not 0 <= int(logprobs) <= MAX_LOGPROBS:
             raise ValueError(f"logprobs must be in [0, {MAX_LOGPROBS}]")
+        seed, frequency_penalty, presence_penalty, logit_bias = check_sampling_params(
+            seed, frequency_penalty, presence_penalty, logit_bias, self.loader.config.get("vocab_size"))
         if len(token_ids) == 0:
             raise ValueError("empty prompt: there is no position to sample the first token from")
         vocab = self.loader.config.get("vocab_size")
@@ -227,7 +275,8 @@ class LLM:
                        self.default_top_p if top_p is None else top_p,
                        1 if top_k is None else top_k,
                        self.default_repetition_penalty if repetition_penalty is None else repetition_penalty,
-                       mm_contents, -1 if logprobs is None else int(logprobs))
+                       mm_contents, -1 if logprobs is None else int(logprobs), seed, frequency_penalty,
+                       presence_penalty, logit_bias)
         if output_len is None:
             seq.output_len = min(4096, self.model_max_length - len(token_ids))
         if mm_contents:
@@ -325,13 +374,16 @@ class LLM:
     def generate(self, prompts: Optional[List[str]] = None, tokens: Optional[List[List[int]]] = None,
                  output_lens: Optional[List[int]] = None, temperature=None, top_p=None, top_k=None,
                  repetition_penalty=None, ignore_eos: bool = False, progress: bool = False,
-                 mm_contents: Optional[List[Optional[dict]]] = None, logprobs=None) -> List[Sequence]:
+                 mm_contents: Optional[List[Optional[dict]]] = None, logprobs=None, seed=None,
+                 frequency_penalty=None, presence_penalty=None, logit_bias=None) -> List[Sequence]:
         """Batch generation; returns the finished `Sequence`s in request order with `.prompt`,
         `.output`, `.token_ids` (reference: gllm/llm_engine.py:343-378). `mm_contents[i]` (VL models) is
         the processor output of request i: pixel_values / image_grid_thw [/ pixel_values_videos ...].
         `logprobs` (None or N in [0, 20], one value or one per request): every generated token gets an entry
         (its log-prob, [(token, log-prob) of the N most likely tokens]) in `.output_logprobs`, under the raw model
-        distribution (log_softmax of the logits, before penalty / temperature / top-k / top-p)."""
+        distribution (log_softmax of the logits, before penalty / temperature / top-k / top-p).
+        `seed`, `frequency_penalty`, `presence_penalty`, `logit_bias` ({token id: bias}): OpenAI sampling parameters,
+        one value or one per request like the others (a dict is one value for all requests)."""
         if self.worker is not None and self.worker.rank != 0:
             return self._serve_until_stop()
         if tokens is None:
@@ -348,7 +400,9 @@ class LLM:
                 return v[i] if isinstance(v, (list, tuple)) else v
             seqs.append(self.allocate_seq(toks, ol, ignore_eos, pick(temperature), pick(top_p), pick(top_k),
                                           pick(repetition_penalty),
-                                          mm_contents[i] if mm_contents is not None else None, pick(logprobs)))
+                                          mm_contents[i] if mm_contents is not None else None, pick(logprobs),
+                                          pick(seed), pick(frequency_penalty), pick(presence_penalty),
+                                          pick(logit_bias)))
         self.add_requests(seqs)
         base = len(self.finished)
         bar = None

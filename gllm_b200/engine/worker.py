@@ -57,7 +57,7 @@ class Worker(ProfilerMixin):
         self.frontend_out: Deque[IPCPackage] = deque()  # in-proc front-end mailbox
         self.frontend_in: Deque[IPCPackage] = deque()
         self.stop = False
-        self._seq_slots = {}                   # seq_id -> row of the penalty state it holds
+        self._seq_slots = {}                   # seq_id -> row of the penalty / bias state it holds
         self._free_slots = []                  # rows given back (row 0 = "no penalty state")
         self._num_slots = 1
         self._penalty_seen = False
@@ -105,7 +105,7 @@ class Worker(ProfilerMixin):
             if pkg.schedule_lists:
                 for seq in pkg.schedule_lists:
                     seq.slot = 0        # penalty state rows are assigned at the first emission (`_assign_slots`)
-                    if seq.repetition_penalty != 1.0:
+                    if seq.repetition_penalty != 1.0 or seq.has_bias_row:
                         self._penalty_seen = True
                 self.scheduler.add_new_requests(pkg.schedule_lists)
             if pkg.abort_ids:
@@ -174,15 +174,16 @@ class Worker(ProfilerMixin):
         return did
 
     def _assign_slots(self, entries):
-        """Penalty state (the per-sequence seen-token bitmask on the device) is held only by sequences that are
-        sampling: a row is assigned when a sequence first emits and returned when it finishes, is aborted or is
-        preempted — never by waiting requests, whose number is unbounded. The pool grows on demand (the runner
-        grows the device tensor to match), so this cannot fail on the request path."""
+        """Penalty state (the per-sequence seen-token bitmask and the frequency / presence / logit_bias row on the
+        device) is held only by sequences that are sampling: a row is assigned when a sequence first emits and
+        returned when it finishes, is aborted or is preempted — never by waiting requests, whose number is unbounded.
+        The pool grows on demand (the runner grows the device tensors to match), so this cannot fail on the request
+        path."""
         if not self._penalty_seen:
-            return          # no request with a repetition penalty has arrived yet: nothing to scan per step
+            return          # no request with a penalty or logit_bias has arrived yet: nothing to scan per step
         for e in entries:
             seq = e.seq
-            if e.emits and seq.repetition_penalty != 1.0 and seq.slot <= 0:
+            if e.emits and (seq.repetition_penalty != 1.0 or seq.has_bias_row) and seq.slot <= 0:
                 if self._free_slots:
                     seq.slot = self._free_slots.pop()
                 else:

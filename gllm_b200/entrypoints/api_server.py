@@ -61,6 +61,17 @@ def _validate_logprobs(request, chat: bool):
     return None
 
 
+def _check_params(request):
+    """-> (error message or None, kwargs of the OpenAI sampling parameters for add_requests_async)."""
+    from gllm_b200.engine.llm_engine import check_sampling_params
+    try:
+        seed, f, p, lb = check_sampling_params(request.seed, request.frequency_penalty, request.presence_penalty,
+                                               request.logit_bias, llm.loader.config.get("vocab_size"))
+    except (ValueError, TypeError) as e:
+        return str(e), None
+    return None, dict(seed=seed, frequency_penalty=f, presence_penalty=p, logit_bias=lb)
+
+
 def _token_str(tok: int) -> str:
     return llm.tokenizer.decode([tok]) if llm.tokenizer is not None else f"token_id:{tok}"
 
@@ -255,7 +266,8 @@ def build_app(engine):
                 token_ids = await _in_thread(llm.encode, None, True, request.messages)
         except Exception as e:  # noqa: BLE001
             return _error(f"cannot encode messages: {e}")
-        bad = _validate_sampling(request) or _validate_logprobs(request, chat=True) or \
+        bad, params = _check_params(request)
+        bad = bad or _validate_sampling(request) or _validate_logprobs(request, chat=True) or \
             _validate(token_ids, request.output_len(), llm.loader.config.get("vocab_size"))
         if bad:
             return _error(bad)
@@ -264,7 +276,8 @@ def build_app(engine):
         stream = await llm.add_requests_async(raw_request, token_ids, request.output_len(), request.ignore_eos,
                                               request.temperature, request.top_p, request.top_k,
                                               request.repetition_penalty, mm_contents, stop=request.stop,
-                                              logprobs=(request.top_logprobs or 0) if request.logprobs else None)
+                                              logprobs=(request.top_logprobs or 0) if request.logprobs else None,
+                                              **params)
         if request.stream:
             return StreamingResponse(chat_completion_stream_generator(stream, request),
                                      media_type="text/event-stream")
@@ -276,7 +289,8 @@ def build_app(engine):
             token_ids = await _in_thread(_encode_prompt, request.prompt)
         except Exception as e:  # noqa: BLE001
             return _error(f"cannot encode prompt: {e}")
-        bad = _validate_sampling(request) or _validate_logprobs(request, chat=False) or \
+        bad, params = _check_params(request)
+        bad = bad or _validate_sampling(request) or _validate_logprobs(request, chat=False) or \
             _validate(token_ids, request.max_tokens, llm.loader.config.get("vocab_size"))
         if bad:
             return _error(bad)
@@ -285,7 +299,7 @@ def build_app(engine):
         stream = await llm.add_requests_async(raw_request, token_ids, request.max_tokens, request.ignore_eos,
                                               request.temperature, request.top_p, request.top_k,
                                               request.repetition_penalty, stop=request.stop,
-                                              logprobs=request.logprobs)
+                                              logprobs=request.logprobs, **params)
         if request.stream:
             return StreamingResponse(completion_stream_generator(stream, request), media_type="text/event-stream")
         return JSONResponse(content=(await completion_generator(stream, request)).model_dump())

@@ -9,9 +9,24 @@ distribution: log_softmax in fp32 of the logits the LM head produced, over the r
 penalty, temperature, top-k and top-p. So they do not depend on the sampling parameters, and the sampled token's
 log-prob is reported under that distribution even when it was drawn with a temperature or a filter. Every generated
 token gets its log-prob and the N most likely tokens (0 <= N <= 20), ordered by logit, ties to the lower token id; for
-a greedy request the first of them is the sampled token. Prompt tokens get none (`echo` is ignored). Token strings are
-`tokenizer.decode([id])` (`bytes`: its UTF-8 encoding), or "token_id:<id>" without a tokenizer. A log-prob of -inf is
-reported as -9999.0. Out-of-range `top_logprobs` / `logprobs`, or `top_logprobs > 0` without `logprobs`, is a 400.
+a greedy request the first of them is the sampled token when it uses no penalty or bias. Prompt tokens get none (`echo`
+is ignored). Token strings are `tokenizer.decode([id])` (`bytes`: its UTF-8 encoding), or "token_id:<id>" without a
+tokenizer. A log-prob of -inf is reported as -9999.0. Out-of-range `top_logprobs` / `logprobs`, or `top_logprobs > 0` without `logprobs`, is a 400.
+
+`frequency_penalty`, `presence_penalty` and `logit_bias` follow OpenAI's formula. For a generated token, with x the
+raw LM-head logit of token j:
+
+    x1 = repetition_penalty(x)            # multiplicative, over prompt + output, as before
+    x2 = x1 - frequency_penalty * c_j - presence_penalty * [c_j > 0] + logit_bias_j
+    t  = x2 / temperature                 # then top-k -> top-p -> draw
+
+c_j counts the occurrences of token j among the tokens this request has generated so far (prompt tokens do not
+count). A greedy request (top_k == 1) takes the argmax of x2, ties to the lower token id. `seed`: a seeded request
+keys its random draw by (seed, index in the sequence of the token being produced, token id), so given the same logits
+it draws the same token whatever the batch, its row in it, the engine's step count, CUDA graphs, lookahead, preemption
+or the tensor-parallel degree; without a seed the draw comes from the engine's own stream. A 400 answers: a penalty
+outside [-2, 2] or not finite; a logit_bias key that is not an int in [0, vocab_size), a value outside [-100, 100] or
+not finite, or more than 1024 entries (this engine's own cap); a seed that does not fit a signed 64-bit int.
 """
 from __future__ import annotations
 

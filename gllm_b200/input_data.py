@@ -60,6 +60,24 @@ class BatchArrays:
     feed_src: Optional[np.ndarray] = None
     # int32 [E]: top alternatives whose log-probs each emitting row wants (-1: none); None when no row asks
     logprobs_n: Optional[np.ndarray] = None
+    # frequency / presence penalties and logit_bias (None unless `need_bias`): per emitting row the penalties and the
+    # slot of its bias row on the device (-1: none)
+    need_bias: bool = False
+    freq_pen: Optional[np.ndarray] = None    # float32 [E]
+    pres_pen: Optional[np.ndarray] = None    # float32 [E]
+    bias_slot: Optional[np.ndarray] = None   # int32 [E]
+    # bias rows to rebuild first (slot (re)assigned): slot, (frequency, presence), the request's logit_bias entries and
+    # the output tokens generated so far, concatenated with [R + 1] offsets
+    rb_slots: Optional[np.ndarray] = None    # int32 [R]
+    rb_pen: Optional[np.ndarray] = None      # float32 [R, 2]
+    rb_lb_off: Optional[np.ndarray] = None   # int32 [R + 1]
+    rb_lb_ids: Optional[np.ndarray] = None   # int32
+    rb_lb_vals: Optional[np.ndarray] = None  # float32
+    rb_out_off: Optional[np.ndarray] = None  # int32 [R + 1]
+    rb_out_toks: Optional[np.ndarray] = None  # int32
+    # seeded rows (None when no row has a seed): request seed and position of the token being produced (-1: unseeded)
+    seed: Optional[np.ndarray] = None        # int64 [E]
+    seed_pos: Optional[np.ndarray] = None    # int32 [E]
     emit_ids: Optional[list] = None  # driver-local: sequence id per EMITTING entry (order of the sampler output)
     seq_ids: Optional[list] = None  # driver-local: sequence id per row (incremental decode batches); not sent
     pt_gens: Optional[list] = None  # driver-local: Sequence.pt_gen per row when the block table rows were written
@@ -73,10 +91,14 @@ class BatchArrays:
         (16-byte aligned sections) so a batch costs two zmq frames per peer instead of one per array."""
         names = ["tokens", "positions", "slot_mapping", "block_table", "seq_lens", "query_start_loc",
                  "logits_idx", "emit_seq", "temperature", "top_k", "top_p", "rep_penalty", "state_slot"]
-        opt = ["seen_rows", "seen_tokens", "clear_slots", "feed_src", "logprobs_n"]
-        hdr = {"scalars": (self.num_decode_seqs, self.num_seqs, self.num_tokens, self.max_q_len,
-                           self.max_seq_len, self.all_greedy, self.need_penalty, self.batch_id),
-               "arrays": [], "mm": self.mm}
+        opt = ["seen_rows", "seen_tokens", "clear_slots", "feed_src", "logprobs_n", "freq_pen", "pres_pen",
+               "bias_slot", "rb_slots", "rb_pen", "rb_lb_off", "rb_lb_ids", "rb_lb_vals", "rb_out_off", "rb_out_toks",
+               "seed", "seed_pos"]
+        scalars = (self.num_decode_seqs, self.num_seqs, self.num_tokens, self.max_q_len, self.max_seq_len,
+                   self.all_greedy, self.need_penalty, self.batch_id)
+        if self.need_bias:      # (only then: a batch without the feature sends the header it always sent)
+            scalars += (True,)
+        hdr = {"scalars": scalars, "arrays": [], "mm": self.mm}
         parts, off = [], 0
         for n in names + opt:
             a = getattr(self, n)
@@ -102,7 +124,8 @@ class BatchArrays:
                 kw[n] = np.frombuffer(blob, dtype=_WIRE_DTYPES[dt], count=math.prod(shape), offset=off).reshape(shape)
         s = hdr["scalars"]
         return BatchArrays(**kw, num_decode_seqs=s[0], num_seqs=s[1], num_tokens=s[2], max_q_len=s[3],
-                           max_seq_len=s[4], all_greedy=s[5], need_penalty=s[6], batch_id=s[7], mm=hdr.get("mm"))
+                           max_seq_len=s[4], all_greedy=s[5], need_penalty=s[6], batch_id=s[7], mm=hdr.get("mm"),
+                           need_bias=len(s) > 8 and s[8])
 
 
 def _page_array(seq) -> np.ndarray:
@@ -164,6 +187,20 @@ def _build_decode_fast(entries, page_size: int, batch_id: int, prev: "BatchArray
     lp_n = prev.logprobs_n[perm] if prev.logprobs_n is not None else None
     if lp_n is not None and not (lp_n >= 0).any():
         lp_n = None        # the rows that asked have finished: the batch is what it would be without the feature
+    bias = {}
+    if prev.need_bias:
+        if any(e.seq.slot_fresh for e in entries):
+            return None    # a bias row to rebuild: the full path sends it
+        bslot = prev.bias_slot[perm]
+        if (bslot >= 0).any():
+            bias = dict(need_bias=True, bias_slot=bslot, freq_pen=prev.freq_pen[perm], pres_pen=prev.pres_pen[perm])
+    seed = seed_pos = None
+    if prev.seed_pos is not None:
+        seed_pos = prev.seed_pos[perm]
+        if (seed_pos >= 0).any():
+            seed, seed_pos = prev.seed[perm], np.where(seed_pos >= 0, seed_pos + 1, -1).astype(np.int32)
+        else:
+            seed_pos = None
     return BatchArrays(feed_src=feed,
         tokens=tokens, positions=starts, slot_mapping=slots.astype(np.int32), block_table=bt, seq_lens=seq_lens,
         query_start_loc=prev.query_start_loc[:b + 1], logits_idx=prev.logits_idx[:b], emit_seq=prev.emit_seq[:b],
@@ -171,7 +208,20 @@ def _build_decode_fast(entries, page_size: int, batch_id: int, prev: "BatchArray
         rep_penalty=prev.rep_penalty[perm], state_slot=prev.state_slot[perm],
         logprobs_n=lp_n, num_decode_seqs=b, num_seqs=b, num_tokens=b, max_q_len=1,
         max_seq_len=int(seq_lens.max()), all_greedy=prev.all_greedy, need_penalty=False, batch_id=batch_id,
-        seq_ids=ids, emit_ids=ids, pt_gens=gens)
+        seq_ids=ids, emit_ids=ids, pt_gens=gens, seed=seed, seed_pos=seed_pos, **bias)
+
+
+def _bias_fields(freq_pen, pres_pen, bias_slot, rb_slots, rb_pen, rb_lb_off, rb_lb_ids, rb_lb_vals, rb_out_off,
+                 rb_out_toks) -> dict:
+    out = dict(need_bias=True, freq_pen=np.asarray(freq_pen, dtype=np.float32),
+               pres_pen=np.asarray(pres_pen, dtype=np.float32), bias_slot=np.asarray(bias_slot, dtype=np.int32))
+    if rb_slots:
+        out.update(rb_slots=np.asarray(rb_slots, dtype=np.int32), rb_pen=np.asarray(rb_pen, dtype=np.float32),
+                   rb_lb_off=np.asarray(rb_lb_off, dtype=np.int32), rb_lb_ids=np.asarray(rb_lb_ids, dtype=np.int32),
+                   rb_lb_vals=np.asarray(rb_lb_vals, dtype=np.float32),
+                   rb_out_off=np.asarray(rb_out_off, dtype=np.int32),
+                   rb_out_toks=np.asarray(rb_out_toks, dtype=np.int32))
+    return out
 
 
 def build_batch(entries, page_size: int, vocab_size: int, batch_id: int = 0, mrope: bool = False,
@@ -206,6 +256,9 @@ def build_batch(entries, page_size: int, vocab_size: int, batch_id: int = 0, mro
     seen_rows, seen_tokens, clear_slots = [], [], []
     logprobs_n, want_logprobs = [], False
     all_greedy, need_penalty = True, False
+    freq_pen, pres_pen, bias_slot, need_bias = [], [], [], False
+    rb_slots, rb_pen, rb_lb_ids, rb_lb_vals, rb_out_toks, rb_lb_off, rb_out_off = [], [], [], [], [], [0], [0]
+    seeds, seed_pos, want_seed = [], [], False
     for i, e in enumerate(entries):
         seq = e.seq
         pt = _page_array(seq)
@@ -244,12 +297,39 @@ def build_batch(entries, page_size: int, vocab_size: int, batch_id: int = 0, mro
                 want_logprobs = True
             if top_k[-1] != 1:
                 all_greedy = False
+            # the state row was just (re)assigned — first emission, or first one after a preemption: its contents are
+            # rebuilt from everything known so far
+            fresh = seq.slot_fresh
+            seq.slot_fresh = False
+            if seq.seed is not None:
+                want_seed = True
+                seeds.append(seq.seed)
+                seed_pos.append(s0 + e.n)          # index of the token this step produces
+            else:
+                seeds.append(0)
+                seed_pos.append(-1)
+            if seq.has_bias_row:
+                need_bias = True
+                bias_slot.append(seq.slot)
+                freq_pen.append(seq.frequency_penalty)
+                pres_pen.append(seq.presence_penalty)
+                if fresh:
+                    rb_slots.append(seq.slot)
+                    rb_pen.append((seq.frequency_penalty, seq.presence_penalty))
+                    lb = seq.logit_bias or {}
+                    rb_lb_ids.extend(lb.keys())
+                    rb_lb_vals.extend(lb.values())
+                    rb_lb_off.append(len(rb_lb_ids))
+                    rb_out_toks.extend(seq.token_ids[seq.prompt_len:s0 + e.n])
+                    rb_out_off.append(len(rb_out_toks))
+            else:
+                bias_slot.append(-1)
+                freq_pen.append(0.0)
+                pres_pen.append(0.0)
             if seq.repetition_penalty != 1.0:
                 need_penalty = True
-                if seq.slot_fresh:
-                    # the row was just (re)assigned — first emission, or first one after a preemption: everything
-                    # known so far (prompt and the tokens generated before) becomes "seen"
-                    seq.slot_fresh = False
+                if fresh:
+                    # everything known so far (prompt and the tokens generated before) becomes "seen"
                     clear_slots.append(seq.slot)
                     seen_rows.append(np.full(s0 + e.n, seq.slot, dtype=np.int32))
                     seen_tokens.append(np.asarray(seq.token_ids[:s0 + e.n], dtype=np.int32))
@@ -272,6 +352,10 @@ def build_batch(entries, page_size: int, vocab_size: int, batch_id: int = 0, mro
         seen_tokens=np.concatenate(seen_tokens) if seen_tokens else None,
         clear_slots=np.asarray(clear_slots, dtype=np.int32) if clear_slots else None, batch_id=batch_id, mm=mm,
         logprobs_n=np.asarray(logprobs_n, dtype=np.int32) if want_logprobs else None,
+        seed=np.asarray(seeds, dtype=np.int64) if want_seed else None,
+        seed_pos=np.asarray(seed_pos, dtype=np.int32) if want_seed else None,
+        **(_bias_fields(freq_pen, pres_pen, bias_slot, rb_slots, rb_pen, rb_lb_off, rb_lb_ids, rb_lb_vals, rb_out_off,
+                        rb_out_toks) if need_bias else {}),
         seq_ids=[e.seq.seq_id for e in entries] if n_dec == b else None,
         pt_gens=[e.seq.pt_gen for e in entries] if n_dec == b else None,
         emit_ids=[entries[i].seq.seq_id for i in emit_seq])
@@ -313,6 +397,11 @@ class InputData:
         self._state_slot = buf((max_seqs,), i32)
         self._tok_seq = buf((max_tokens,), i32)
         self._feed = buf((max_seqs,), i32)
+        self._freq_pen = buf((max_seqs,), f32)
+        self._pres_pen = buf((max_seqs,), f32)
+        self._bias_slot = buf((max_seqs,), i32)
+        self._seed = buf((max_seqs,), torch.int64)
+        self._seed_pos = buf((max_seqs,), i32)
         self.need_tok_seq = False  # MLA attention wants token -> sequence for mixed / prefill batches
         self.batch: Optional[BatchArrays] = None
         self.num_tokens = self.num_seqs = self.num_decode_seqs = self.num_emit = 0
@@ -363,12 +452,20 @@ class InputData:
         if self.num_emit:
             self._put(self._logits_idx, batch.logits_idx)
             # the greedy argmax path of the sm_90a sampler reads none of these
-            if not (self.device.type == "cuda" and batch.all_greedy and not batch.need_penalty):
+            if not (self.device.type == "cuda" and batch.all_greedy and not batch.need_penalty and not batch.need_bias):
                 self._put(self._temperature, batch.temperature)
                 self._put(self._top_k, batch.top_k)
                 self._put(self._top_p, batch.top_p)
                 self._put(self._rep_penalty, batch.rep_penalty)
                 self._put(self._state_slot, batch.state_slot)
+            # per-request sampling parameters: staged only when some row uses them
+            if batch.need_bias:
+                self._put(self._freq_pen, batch.freq_pen)
+                self._put(self._pres_pen, batch.pres_pen)
+                self._put(self._bias_slot, batch.bias_slot)
+            if batch.seed is not None:
+                self._put(self._seed, batch.seed)
+                self._put(self._seed_pos, batch.seed_pos)
 
     def apply_feed(self, prev_tokens_out: torch.Tensor):
         """Lookahead step: the input tokens are the previous step's sampled tokens, still on the device."""
@@ -448,6 +545,24 @@ class InputData:
     @property
     def state_slot(self): return self._state_slot[1][: self.num_emit]
 
+    @property
+    def freq_pen(self): return self._freq_pen[1][: self.num_emit]
+
+    @property
+    def pres_pen(self): return self._pres_pen[1][: self.num_emit]
+
+    @property
+    def bias_slot(self):
+        """int32 [E] bias row of each emitting row (-1: none), or None when no row of the batch has one."""
+        return self._bias_slot[1][: self.num_emit] if self.batch is not None and self.batch.need_bias else None
+
+    @property
+    def seeds(self):
+        """(int64 seeds [E], int32 positions [E]) of a batch with seeded rows, else (None, None)."""
+        if self.batch is None or self.batch.seed is None:
+            return None, None
+        return self._seed[1][: self.num_emit], self._seed_pos[1][: self.num_emit]
+
     def h2d_bytes(self) -> int:
         b = self.batch
         if b is None:
@@ -456,4 +571,7 @@ class InputData:
         for a in (b.tokens, b.positions, b.slot_mapping, b.block_table, b.seq_lens, b.query_start_loc,
                   b.logits_idx, b.temperature, b.top_k, b.top_p, b.rep_penalty, b.state_slot):
             tot += a.nbytes
+        for a in (b.freq_pen, b.pres_pen, b.bias_slot, b.seed, b.seed_pos):
+            if a is not None:
+                tot += a.nbytes
         return tot

@@ -91,6 +91,8 @@ class ModelRunner:
         self.num_pages = 0
         self.device = None
         self.seen_bits = None
+        self.bias_rows = None    # fp32 [slots, V]: frequency / presence penalties + logit_bias (`_bias_state`)
+        self.out_seen = None     # int32 [slots, ceil(V/32)]: tokens each slot's sequence has generated
         self.step_counter = None
         self.stats = {"steps": 0, "graph_steps": 0, "tokens": 0, "h2d_bytes": 0, "d2h_bytes": 0,
                       "graph_kernel_launches": 0, "gpu_ms": 0.0}
@@ -281,6 +283,7 @@ class ModelRunner:
         inp.load(batch)
         if batch.feed_src is not None:
             inp.apply_feed(self.tokens_out)
+            self.stats["feed_steps"] = self.stats.get("feed_steps", 0) + 1     # lookahead steps
         self.stats["h2d_bytes"] += inp.h2d_bytes()
         if self.time_steps and self.device.type == "cuda":
             ev0 = torch.cuda.Event(enable_timing=True)
@@ -343,7 +346,12 @@ class ModelRunner:
         if self.keep_logits:
             full = self.tpc.gather_logits(logits, self.spec.vocab_size) if self.vp_sample else logits
             self.logit_log.append((list(batch.emit_ids or []), full[:e, : self.spec.vocab_size].float().cpu()))
-        if self.vp_sample and batch.all_greedy and not batch.need_penalty:
+        bias = None
+        if batch.need_bias:
+            bias = self._bias_state(int(batch.bias_slot.max()) + 1)
+            if batch.rb_slots is not None:
+                self._rebuild_bias(batch)
+        if self.vp_sample and batch.all_greedy and not batch.need_penalty and not batch.need_bias:
             toks = self._vp_greedy(logits)
             return self._finish_sample(toks, e, self._logprobs(batch, logits, toks, vocab_parallel=True))
         if self.vp_sample and not self.vp_candidates:
@@ -368,10 +376,60 @@ class ModelRunner:
         if not batch.all_greedy:
             self.step_counter += 1
         if self.vp_sample and self.vp_candidates:
-            toks = self._vp_sample(logits, seen)
+            toks = self._vp_sample(logits, seen, bias)
+            self._account_bias(batch, toks)
             return self._finish_sample(toks, e, self._logprobs(batch, logits, toks, vocab_parallel=True))
-        toks = Fn.sample(logits, inp, seen, seed=self.cfg.seed, step=self.step_counter)
+        toks = Fn.sample(logits, inp, seen, seed=self.cfg.seed, step=self.step_counter, bias_rows=bias)
+        self._account_bias(batch, toks)
         return self._finish_sample(toks, e, self._logprobs(batch, logits, toks, vocab_parallel=False))
+
+    def _bias_state(self, rows: int) -> torch.Tensor:
+        """[rows, V] fp32 bias rows (and the [rows, V/32] output-token bitmask), one per slot; grown (never shrunk)
+        like `_seen_bits`. About V * 4.125 bytes per slot (594 KiB at V = 151936); not part of the KV-cache sizing."""
+        if self.bias_rows is None or self.bias_rows.shape[0] < rows:
+            v = self.spec.vocab_size
+            n = max(rows, 65 if self.bias_rows is None else 2 * self.bias_rows.shape[0])
+            b = torch.zeros(n, v, dtype=torch.float32, device=self.device)
+            o = torch.zeros(n, (v + 31) // 32, dtype=torch.int32, device=self.device)
+            if self.bias_rows is not None:
+                b[: self.bias_rows.shape[0]] = self.bias_rows
+                o[: self.out_seen.shape[0]] = self.out_seen
+            self.bias_rows, self.out_seen = b, o
+        return self.bias_rows
+
+    def _rebuild_bias(self, batch: BatchArrays):
+        """Slots (re)assigned this step: clear, scatter logit_bias, replay the counts of the outputs known so far."""
+        dev = self.device
+        if dev.type == "cuda":
+            from gllm_b200.ops import sm100
+            t = [torch.from_numpy(np.ascontiguousarray(a)).to(dev) for a in
+                 (batch.rb_slots, batch.rb_pen, batch.rb_lb_off, batch.rb_lb_ids, batch.rb_lb_vals, batch.rb_out_off,
+                  batch.rb_out_toks)]
+            sm100.bias_rebuild(self.bias_rows, self.out_seen, self.spec.vocab_size, *t)
+            return
+        from gllm_b200.ops import ref
+        lo, oo = batch.rb_lb_off, batch.rb_out_off
+        for r, slot in enumerate(batch.rb_slots.tolist()):
+            ref.bias_rebuild(self.bias_rows, self.out_seen, slot, float(batch.rb_pen[r, 0]), float(batch.rb_pen[r, 1]),
+                             batch.rb_lb_ids[lo[r]:lo[r + 1]], batch.rb_lb_vals[lo[r]:lo[r + 1]],
+                             batch.rb_out_toks[oo[r]:oo[r + 1]].tolist())
+
+    def _account_bias(self, batch: BatchArrays, toks: torch.Tensor):
+        """After the tokens are chosen: every emitting row with a bias row charges its token, on the device — the host
+        never sends per-step tokens, so these rows stay eligible for lookahead and the incremental decode path."""
+        if not batch.need_bias:
+            return
+        inp = self.input_data
+        if toks.is_cuda:
+            from gllm_b200.ops import sm100
+            sm100.bias_account(self.bias_rows, self.out_seen, inp.bias_slot, toks.to(torch.int32).contiguous(),
+                               inp.freq_pen, inp.pres_pen)
+            return
+        from gllm_b200.ops import ref
+        for r, (slot, tok) in enumerate(zip(inp.bias_slot.tolist(), toks.tolist())):
+            if slot >= 0:
+                ref.bias_account_one(self.bias_rows, self.out_seen, slot, int(tok), float(inp.freq_pen[r]),
+                                     float(inp.pres_pen[r]))
 
     def _logprobs(self, batch: BatchArrays, logits: torch.Tensor, toks: torch.Tensor,
                   vocab_parallel: bool) -> Optional[torch.Tensor]:
@@ -412,7 +470,8 @@ class ModelRunner:
 
     VP_CANDIDATES = 256   # per rank and row; top_k <= this is exact (csrc/sample/sampler.cu)
 
-    def _vp_sample(self, shard: torch.Tensor, seen: Optional[torch.Tensor]) -> torch.Tensor:
+    def _vp_sample(self, shard: torch.Tensor, seen: Optional[torch.Tensor],
+                   bias: Optional[torch.Tensor] = None) -> torch.Tensor:
         """Vocab-parallel top-k / top-p / penalty sampling (SURVEY §2.4 X4): every rank reduces its vocab shard to
         a [E, 2C+4] record (C best candidates, softmax statistics, race winner), the ranks all-gather the records —
         ~2 KB per row and rank instead of V/tp logits — and finish on the tp x C candidates with the exact global
@@ -427,16 +486,25 @@ class ModelRunner:
         valid = max(0, min(per, v_full - r0))
         c = min(self.VP_CANDIDATES, per)
         pen = inp.rep_penalty[:e] if seen is not None else None
+        seeds, spos = inp.seeds
+        bslot = inp.bias_slot if bias is not None else None
         if shard.is_cuda:
             from gllm_b200.ops import sm100
             rec = sm100.vp_candidates(shard, valid, v_full, c, inp.temperature[:e], inp.top_k[:e], inp.top_p[:e],
                                       pen, seen, inp.state_slot[:e] if seen is not None else None,
-                                      seed=self.cfg.seed, step=self.step_counter, vocab_offset=r0)
+                                      seed=self.cfg.seed, step=self.step_counter, vocab_offset=r0,
+                                      bias=bias if bslot is not None else None, bias_slot=bslot, seeds=seeds,
+                                      seed_pos=spos)
         else:
             from gllm_b200.ops import ref
             step = int(self.step_counter) if self.step_counter is not None else 0
             g = torch.Generator().manual_seed(self.cfg.seed + step)
             race = torch.empty(e, per * st.tp_size).exponential_(1.0, generator=g)[:, r0:r0 + max(valid, 0)]
+            if seeds is not None:       # seeded rows: the kernel's stream, keyed by token id
+                for r in np.nonzero(spos.numpy() >= 0)[0].tolist():
+                    race[r] = ref.race_exp(int(seeds[r]), int(spos[r]), range(r0, r0 + max(valid, 0)))
+            dense = _dense_bias(bias, bslot, r0 + max(valid, 0))
+            dense = dense[:, r0:] if dense is not None else None
             mask = None
             if seen is not None:
                 rows = seen[inp.state_slot[:e].long()]
@@ -446,15 +514,15 @@ class ModelRunner:
                     full = torch.nn.functional.pad(full, (0, r0 + valid - full.shape[1]))
                 mask = full[:, r0:r0 + valid]
             rec = ref.vp_candidates(shard, valid, v_full, c, inp.temperature[:e], inp.top_k[:e], inp.top_p[:e], pen,
-                                    mask, race, vocab_offset=r0)
+                                    mask, race, vocab_offset=r0, bias=dense)
         allr = torch.empty(st.tp_size, e, 2 * c + 4, dtype=torch.float32, device=shard.device)
         dist.all_gather_into_tensor(allr.view(st.tp_size * e, 2 * c + 4), rec, group=st.tp_group)
         self.stats["vp_sample_steps"] = self.stats.get("vp_sample_steps", 0) + 1
         if shard.is_cuda:
             return sm100.vp_final(allr, c, v_full, inp.top_k[:e], inp.top_p[:e], seed=self.cfg.seed,
-                                  step=self.step_counter)
+                                  step=self.step_counter, seeds=seeds, seed_pos=spos)
         g = torch.Generator().manual_seed(self.cfg.seed + step + 0x5bd1)
-        return ref.vp_final(allr, c, v_full, inp.top_k[:e], inp.top_p[:e], generator=g)
+        return ref.vp_final(allr, c, v_full, inp.top_k[:e], inp.top_p[:e], generator=g, seeds=seeds, seed_pos=spos)
 
     def _vp_greedy(self, shard: torch.Tensor) -> torch.Tensor:
         """Vocab-parallel greedy sampling (SURVEY §2.4 X4): every rank takes the argmax of its own vocab shard
@@ -532,6 +600,15 @@ class ModelRunner:
                 new[: self.seen_bits.shape[0]] = self.seen_bits
             self.seen_bits = new
         return self.seen_bits
+
+
+def _dense_bias(bias_rows: Optional[torch.Tensor], bias_slot: Optional[torch.Tensor], v: int):
+    """CPU path: [E, v] additive rows of the emitting rows (zeros where a row has none), or None."""
+    if bias_rows is None or bias_slot is None:
+        return None
+    rows = bias_rows[bias_slot.clamp(min=0).long(), :v].clone()
+    rows[bias_slot < 0] = 0.0
+    return rows
 
 
 def _dummy_batch(num_tokens: int, num_seqs: int, page_size: int, max_blocks: int, page: int = 0,

@@ -67,10 +67,12 @@ def _declare(lib):
     sig("gllm_attn_prefill_tc", [P, L, P, P, P, L, P, P, P, I, I, I, I, I, I, I, I, F, I, P])
     sig("gllm_mla_attention", [P, P, P, L, P, P, P, P, P, I, I, I, I, I, F, P])
     sig("gllm_mla_rope_cache", [P, L, L, I, P, P, L, P, L, P, P, P, P, I, I, P])
-    sig("gllm_sample", [P, I, L, P, I, I, P, P, P, P, P, I, P, c_uint64, P, P, I, P])
+    sig("gllm_sample", [P, I, L, P, I, I, P, P, P, P, P, I, P, c_uint64, P, P, I, P, L, P, P, P, P])
     sig("gllm_mark_seen", [P, I, P, P, I, P])
-    sig("gllm_vp_candidates", [P, I, L, P, I, I, I, I, P, P, P, P, P, I, P, c_uint64, P, I, P])
-    sig("gllm_vp_final", [P, I, I, I, I, P, P, c_uint64, P, P, P])
+    sig("gllm_vp_candidates", [P, I, L, P, I, I, I, I, P, P, P, P, P, I, P, c_uint64, P, I, P, L, P, P, P, P])
+    sig("gllm_vp_final", [P, I, I, I, I, P, P, c_uint64, P, P, P, P, P])
+    sig("gllm_bias_account", [P, L, P, I, P, P, P, P, I, P])
+    sig("gllm_bias_rebuild", [P, L, P, I, I, I, P, P, P, P, P, P, P, P])
     sig("gllm_logprobs_shard", [P, I, L, I, I, I, P, P, P, I, P])
     sig("gllm_logprobs_final", [P, I, I, I, P, P])
     sig("gllm_moe_topk_softmax", [P, L, P, P, I, I, I, I, P])

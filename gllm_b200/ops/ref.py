@@ -230,11 +230,62 @@ def varlen_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, cu_seqle
 # ----------------------------------------------------------------------------------------------
 # sampling
 # ----------------------------------------------------------------------------------------------
-def apply_penalty_temperature(logits: torch.Tensor, temperature, rep_penalty, seen_mask) -> torch.Tensor:
+_M32 = 0xFFFFFFFF
+
+
+def _hash_u32(x):
+    """csrc/sample/sampler.cu:hash_u32 on uint64 numpy arrays holding uint32 values (products wrap mod 2^64, whose
+    low 32 bits are the uint32 product)."""
+    x = x ^ (x >> 16)
+    x = (x * 0x7feb352d) & _M32
+    x = x ^ (x >> 15)
+    x = (x * 0x846ca68b) & _M32
+    return x ^ (x >> 16)
+
+
+def race_uniform(seed: int, row: int, tokens) -> "np.ndarray":
+    """Bit-exact port of the uniform inside csrc/sample/sampler.cu:rand_exp — u in (0, 1), float32, for the
+    exponential race keyed (seed, row, token id). A seeded request row uses (its seed, position of the token being
+    produced); the kernel's exponential variate is -log(u) (fast-math log, so that part agrees to rounding only)."""
+    import numpy as np
+    seed = int(seed) & ((1 << 64) - 1)
+    lo, hi = seed & _M32, seed >> 32
+    t = np.asarray(tokens, dtype=np.int64).astype(np.uint64) & _M32
+    a = _hash_u32(np.asarray([(int(row) * 0x9E3779B9 + 0x85ebca6b) & _M32], dtype=np.uint64))
+    h = _hash_u32((t + ((hi * 0xc2b2ae35) & _M32)) & _M32)
+    h = _hash_u32(np.uint64(lo) ^ a ^ h)
+    h = _hash_u32(h ^ 0x27d4eb2f)
+    return (((h >> 8).astype(np.float32) + np.float32(0.5)) * np.float32(1.0 / 16777216.0)).astype(np.float32)
+
+
+def race_exp(seed: int, row: int, tokens) -> torch.Tensor:
+    """Exponential variates of the seeded race (float32): -log of `race_uniform`."""
+    return -torch.log(torch.from_numpy(race_uniform(seed, row, tokens)))
+
+
+def _seeded_exp(probs_shape, generator, seeds, seed_pos, tokens=None) -> torch.Tensor:
+    """Exp(1) variates [B, n]: from `generator` for unseeded rows, from the seeded race for rows with seed_pos >= 0
+    (`tokens` [B, n] token id of each column; default: the column index)."""
+    b, n = probs_shape
+    g = torch.empty(b, n).exponential_(1.0, generator=generator)
+    if seeds is not None:
+        for r in range(b):
+            pos = int(seed_pos[r])
+            if pos >= 0:
+                tk = tokens[r].cpu().numpy() if tokens is not None else range(n)
+                g[r] = race_exp(int(seeds[r]), pos, list(tk))
+    return g
+
+
+def apply_penalty_temperature(logits: torch.Tensor, temperature, rep_penalty, seen_mask, bias=None) -> torch.Tensor:
+    """`bias`: optional dense fp32 [B, V] additive term (frequency / presence penalties and logit_bias), added after
+    the repetition penalty and before the temperature, as the kernel does."""
     x = logits.float().clone()
     if rep_penalty is not None and seen_mask is not None:
         pen = rep_penalty.view(-1, 1).float()
         x = torch.where(seen_mask, torch.where(x > 0, x / pen, x * pen), x)
+    if bias is not None:
+        x = x + bias.float()
     if temperature is not None:
         t = temperature.float().clone()
         t[t <= 1e-5] = 1.0
@@ -243,10 +294,10 @@ def apply_penalty_temperature(logits: torch.Tensor, temperature, rep_penalty, se
 
 
 def sample_filter(logits: torch.Tensor, temperature=None, top_k=None, top_p=None, rep_penalty=None,
-                  seen_mask=None) -> torch.Tensor:
+                  seen_mask=None, bias=None) -> torch.Tensor:
     """Returns the filtered probability distribution [B, V] the sampler draws from
     (reference semantics: gllm/layers/sampler.py:22-54)."""
-    x = apply_penalty_temperature(logits, temperature, rep_penalty, seen_mask)
+    x = apply_penalty_temperature(logits, temperature, rep_penalty, seen_mask, bias)
     b, v = x.shape
     if top_k is not None:
         k = top_k.clone().long()
@@ -266,14 +317,17 @@ def sample_filter(logits: torch.Tensor, temperature=None, top_k=None, top_p=None
 
 
 def sample(logits: torch.Tensor, temperature=None, top_k=None, top_p=None, rep_penalty=None,
-           seen_mask=None, generator: Optional[torch.Generator] = None) -> torch.Tensor:
+           seen_mask=None, generator: Optional[torch.Generator] = None, bias=None, seeds=None,
+           seed_pos=None) -> torch.Tensor:
+    """`seeds` / `seed_pos` (int64 / int32 [B]): rows with seed_pos >= 0 draw from the seeded race (`race_exp`), so
+    their token depends on their logits alone, whatever the batch."""
     b, v = logits.shape
     greedy = top_k is None or bool((top_k == 1).all())
     if greedy:
-        x = apply_penalty_temperature(logits, temperature, rep_penalty, seen_mask)
+        x = apply_penalty_temperature(logits, temperature, rep_penalty, seen_mask, bias)
         return x.argmax(-1).to(torch.int32)
-    probs = sample_filter(logits, temperature, top_k, top_p, rep_penalty, seen_mask)
-    g = torch.empty_like(probs).exponential_(1.0, generator=generator)
+    probs = sample_filter(logits, temperature, top_k, top_p, rep_penalty, seen_mask, bias)
+    g = _seeded_exp(probs.shape, generator, seeds, seed_pos)
     tok = (probs / g).argmax(-1)
     # rows with top_k == 1 are exactly greedy
     return tok.to(torch.int32)
@@ -281,11 +335,11 @@ def sample(logits: torch.Tensor, temperature=None, top_k=None, top_p=None, rep_p
 
 def vp_candidates(shard: torch.Tensor, valid: int, v_full: int, c: int, temperature=None, top_k=None, top_p=None,
                   rep_penalty=None, seen_mask=None, race_exp: Optional[torch.Tensor] = None,
-                  vocab_offset: int = 0) -> torch.Tensor:
+                  vocab_offset: int = 0, bias=None) -> torch.Tensor:
     """PyTorch model of csrc/sample/sampler.cu:vp_candidates_kernel — per-row record [B, 2c+4]: the shard's c best
     candidates after penalty / temperature (values, then token ids bit-cast to float), shard max, shard sum-exp, and
     for unfiltered rows the shard's exponential-race winner (score relative to the shard max, token id).
-    `seen_mask` / `race_exp` are [B, valid] slices for this shard."""
+    `seen_mask` / `race_exp` / `bias` are [B, valid] slices for this shard."""
     b = shard.shape[0]
     out = torch.full((b, 2 * c + 4), float("-inf"), dtype=torch.float32)
     out[:, c:2 * c] = 0.0
@@ -293,7 +347,7 @@ def vp_candidates(shard: torch.Tensor, valid: int, v_full: int, c: int, temperat
     out[:, 2 * c + 3] = 0.0
     if valid <= 0:
         return out
-    x = apply_penalty_temperature(shard[:, :valid], temperature, rep_penalty, seen_mask)
+    x = apply_penalty_temperature(shard[:, :valid], temperature, rep_penalty, seen_mask, bias)
     m = x.max(dim=-1).values
     out[:, 2 * c] = m
     out[:, 2 * c + 1] = torch.exp(x - m.view(-1, 1)).sum(-1)
@@ -314,7 +368,7 @@ def vp_candidates(shard: torch.Tensor, valid: int, v_full: int, c: int, temperat
 
 
 def vp_final(gathered: torch.Tensor, c: int, v_full: int, top_k=None, top_p=None,
-             generator: Optional[torch.Generator] = None) -> torch.Tensor:
+             generator: Optional[torch.Generator] = None, seeds=None, seed_pos=None) -> torch.Tensor:
     """PyTorch model of vp_final_kernel: finish top-k / top-p / draw on the gathered candidates [tp, B, 2c+4] with
     the exact global normalisation (the mass of non-candidate tokens is known from the per-shard sum-exp)."""
     tp, b, _ = gathered.shape
@@ -330,6 +384,7 @@ def vp_final(gathered: torch.Tensor, c: int, v_full: int, top_k=None, top_p=None
     out = torch.zeros(b, dtype=torch.int32)
     e_all = torch.empty(b, n).exponential_(1.0, generator=generator)
     for r in range(b):
+        seeded = seeds is not None and int(seed_pos[r]) >= 0
         if k[r] >= v_full and p[r] >= 1.0:
             sc = gathered[:, r, 2 * c + 2] + (ms[:, r] - gm[r])
             out[r] = gathered[int(sc.argmax()), r, 2 * c + 3].view(torch.int32)
@@ -337,6 +392,7 @@ def vp_final(gathered: torch.Tensor, c: int, v_full: int, top_k=None, top_p=None
         x, t = vals[r], toks[r]
         order = torch.argsort(x, descending=True, stable=True)
         x, t = x[order], t[order]
+        e_r = race_exp(int(seeds[r]), int(seed_pos[r]), t.tolist()) if seeded else e_all[r]
         kk = int(min(k[r], n))
         if kk == 1:
             out[r] = t[0]
@@ -351,9 +407,32 @@ def vp_final(gathered: torch.Tensor, c: int, v_full: int, top_k=None, top_p=None
             cum = torch.cumsum(torch.where(keep, prob, torch.zeros_like(prob)), 0)
             keep &= (cum - prob) < p[r] * mass
         keep &= x > float("-inf")
-        score = torch.where(keep, torch.log(prob) - torch.log(e_all[r]), torch.full_like(prob, float("-inf")))
+        score = torch.where(keep, torch.log(prob) - torch.log(e_r), torch.full_like(prob, float("-inf")))
         out[r] = t[int(score.argmax())]
     return out
+
+
+def bias_rebuild(bias: torch.Tensor, out_seen: torch.Tensor, slot: int, freq: float, pres: float, lb_ids, lb_vals,
+                 out_toks):
+    """PyTorch model of bias_rebuild_kernel for one slot: clear, scatter logit_bias, replay the output tokens' counts
+    in order with the fp32 operations of bias_account."""
+    bias[slot] = 0.0
+    out_seen[slot] = 0
+    if len(lb_ids):
+        bias[slot, torch.as_tensor(lb_ids, dtype=torch.long)] = torch.as_tensor(lb_vals, dtype=torch.float32)
+    for tok in out_toks:
+        bias_account_one(bias, out_seen, slot, int(tok), freq, pres)
+
+
+def bias_account_one(bias: torch.Tensor, out_seen: torch.Tensor, slot: int, tok: int, freq: float, pres: float):
+    """PyTorch model of bias_account_kernel for one row: bias[slot, tok] -= f (+ p on the first occurrence)."""
+    w, bit = tok >> 5, 1 << (tok & 31)
+    word = int(out_seen[slot, w]) & _M32
+    first = (word & bit) == 0
+    new = word | bit
+    out_seen[slot, w] = new - (1 << 32) if new >= 1 << 31 else new     # int32 storage of the uint32 word
+    f, p = torch.tensor(freq, dtype=torch.float32), torch.tensor(pres, dtype=torch.float32)
+    bias[slot, tok] = bias[slot, tok] - ((f + p) if first else f)
 
 
 LP_NO_TOKEN = 0x7fffffff   # token id of an empty candidate slot in a log-prob record

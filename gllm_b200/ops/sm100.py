@@ -353,9 +353,13 @@ def sample(logits: torch.Tensor, temperature=None, top_k=None, top_p=None, rep_p
            seen_bits: Optional[torch.Tensor] = None, slot_idx: Optional[torch.Tensor] = None, seed: int = 0,
            step: Optional[torch.Tensor] = None,
            out: Optional[torch.Tensor] = None, out_max: Optional[torch.Tensor] = None,
-           vocab_offset: int = 0) -> torch.Tensor:
+           vocab_offset: int = 0, bias: Optional[torch.Tensor] = None, bias_slot: Optional[torch.Tensor] = None,
+           seeds: Optional[torch.Tensor] = None, seed_pos: Optional[torch.Tensor] = None) -> torch.Tensor:
     """logits [B, V] bf16/fp32; per-row params fp32/int32 tensors or None. seen_bits: uint32/int32
-    bitmask [B, ceil(V/32)] of tokens subject to the repetition penalty."""
+    bitmask [B, ceil(V/32)] of tokens subject to the repetition penalty. bias: fp32 [slots, >= V_full] additive rows
+    (frequency / presence penalties, logit_bias) indexed by token id, bias_slot: int32 [B] row of each batch row (-1:
+    none). seeds: int64 [B] request seeds, seed_pos: int32 [B] position of the token being produced (-1: unseeded
+    row, keyed by `seed` + `step` and the batch row)."""
     assert logits.dim() == 2 and logits.stride(1) == 1
     b, v = logits.shape
     dtype = 0 if logits.dtype == _BF16 else 1
@@ -367,16 +371,28 @@ def sample(logits: torch.Tensor, temperature=None, top_k=None, top_p=None, rep_p
     rc = L.gllm_sample(_p(logits), dtype, logits.stride(0), _p(out), b, v, _p(temperature), _p(top_k), _p(top_p),
                        _p(rep_penalty), _p(seen_bits), seen_words, _p(slot_idx),
                        ctypes.c_uint64(seed & ((1 << 64) - 1)),
-                       _p(step), _p(out_max), vocab_offset, stream_ptr())
+                       _p(step), _p(out_max), vocab_offset, *_bias_seed_args(bias, bias_slot, seeds, seed_pos),
+                       stream_ptr())
     check(rc, "sample")
     _count()
     return out
 
 
+def _bias_seed_args(bias, bias_slot, seeds, seed_pos):
+    if bias is not None:
+        assert bias.dtype == torch.float32 and bias.stride(1) == 1 and bias_slot.dtype == torch.int32
+    if seeds is not None:
+        assert seeds.dtype == torch.int64 and seed_pos.dtype == torch.int32
+    return (_p(bias), bias.stride(0) if bias is not None else 0, _p(bias_slot if bias is not None else None),
+            _p(seeds), _p(seed_pos if seeds is not None else None))
+
+
 def vp_candidates(shard: torch.Tensor, valid: int, v_full: int, c: int, temperature=None, top_k=None, top_p=None,
                   rep_penalty=None, seen_bits: Optional[torch.Tensor] = None,
                   slot_idx: Optional[torch.Tensor] = None, seed: int = 0, step: Optional[torch.Tensor] = None,
-                  vocab_offset: int = 0) -> torch.Tensor:
+                  vocab_offset: int = 0, bias: Optional[torch.Tensor] = None,
+                  bias_slot: Optional[torch.Tensor] = None, seeds: Optional[torch.Tensor] = None,
+                  seed_pos: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Vocab-parallel sampling, stage 1 (csrc/sample/sampler.cu): this rank's per-row record [B, 2c+4] fp32 — its c
     best candidates (value, token id), (max, sum exp) of the shard, and the shard's race winner for unfiltered rows.
     `valid`: columns of `shard` that are real vocabulary entries (the last rank's shard ends with padding)."""
@@ -388,21 +404,23 @@ def vp_candidates(shard: torch.Tensor, valid: int, v_full: int, c: int, temperat
     rc = L.gllm_vp_candidates(_p(shard), 0 if shard.dtype == _BF16 else 1, shard.stride(0), _p(out), b, valid, v_full,
                               c, _p(temperature), _p(top_k), _p(top_p), _p(rep_penalty), _p(seen_bits), seen_words,
                               _p(slot_idx), ctypes.c_uint64(seed & ((1 << 64) - 1)), _p(step), vocab_offset,
-                              stream_ptr())
+                              *_bias_seed_args(bias, bias_slot, seeds, seed_pos), stream_ptr())
     check(rc, "vp_candidates")
     _count()
     return out
 
 
 def vp_final(gathered: torch.Tensor, c: int, v_full: int, top_k=None, top_p=None, seed: int = 0,
-             step: Optional[torch.Tensor] = None) -> torch.Tensor:
+             step: Optional[torch.Tensor] = None, seeds: Optional[torch.Tensor] = None,
+             seed_pos: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Vocab-parallel sampling, stage 2: `gathered` [tp, B, 2c+4] (all ranks' stage-1 records) -> tokens [B]."""
     tp, b, w = gathered.shape
     assert w == 2 * c + 4 and gathered.is_contiguous() and gathered.dtype == torch.float32
     out = torch.empty(b, dtype=torch.int32, device=gathered.device)
     L = _lib.load()
     rc = L.gllm_vp_final(_p(gathered), tp, b, c, v_full, _p(top_k), _p(top_p),
-                         ctypes.c_uint64(seed & ((1 << 64) - 1)), _p(step), _p(out), stream_ptr())
+                         ctypes.c_uint64(seed & ((1 << 64) - 1)), _p(step), _p(out),
+                         *_bias_seed_args(None, None, seeds, seed_pos)[3:], stream_ptr())
     check(rc, "vp_final")
     _count()
     return out
@@ -442,6 +460,35 @@ def logprobs_final(gathered: torch.Tensor, n: int) -> torch.Tensor:
     check(L.gllm_logprobs_final(_p(gathered), tp, e, n, _p(out), stream_ptr()), "logprobs_final")
     _count()
     return out
+
+
+def bias_account(bias: torch.Tensor, out_seen: torch.Tensor, bias_slot: torch.Tensor, tokens: torch.Tensor,
+                 freq: torch.Tensor, pres: torch.Tensor):
+    """Charge each emitting row's sampled token to its bias row (csrc/sample/sampler.cu:bias_account_kernel):
+    bias[slot, tok] -= freq (+ pres the first time), out_seen bit set. bias_slot int32 [E] (-1: no row)."""
+    e = bias_slot.numel()
+    assert tokens.dtype == torch.int32 and tokens.numel() >= e and bias_slot.dtype == torch.int32
+    assert freq.dtype == torch.float32 and pres.dtype == torch.float32 and bias.stride(1) == 1
+    L = _lib.load()
+    check(L.gllm_bias_account(_p(bias), bias.stride(0), _p(out_seen), out_seen.shape[1], _p(bias_slot), _p(tokens),
+                              _p(freq), _p(pres), e, stream_ptr()), "bias_account")
+    _count()
+
+
+def bias_rebuild(bias: torch.Tensor, out_seen: torch.Tensor, v: int, slots: torch.Tensor, pen: torch.Tensor,
+                 lb_off: torch.Tensor, lb_ids: torch.Tensor, lb_vals: torch.Tensor, out_off: torch.Tensor,
+                 out_toks: torch.Tensor):
+    """Rebuild the bias rows of (re)assigned slots (bias_rebuild_kernel): clear, scatter logit_bias, replay the counts
+    of the output tokens in order. pen fp32 [R, 2] (frequency, presence); *_off int32 [R + 1] offsets."""
+    r = slots.numel()
+    for t, dt in ((slots, torch.int32), (pen, torch.float32), (lb_off, torch.int32), (lb_ids, torch.int32),
+                  (lb_vals, torch.float32), (out_off, torch.int32), (out_toks, torch.int32)):
+        assert t.dtype == dt and t.is_contiguous()
+    L = _lib.load()
+    check(L.gllm_bias_rebuild(_p(bias), bias.stride(0), _p(out_seen), out_seen.shape[1], v, r, _p(slots), _p(pen),
+                              _p(lb_off), _p(lb_ids), _p(lb_vals), _p(out_off), _p(out_toks), stream_ptr()),
+          "bias_rebuild")
+    _count()
 
 
 def mark_seen(seen_bits: torch.Tensor, rows: torch.Tensor, tokens: torch.Tensor):

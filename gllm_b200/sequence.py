@@ -1,7 +1,7 @@
 """Per-request state (reference: gllm/sequence.py:8-98)."""
 from __future__ import annotations
 
-from typing import List, Optional
+from typing import Dict, List, Optional
 
 
 class Sequence:
@@ -10,12 +10,14 @@ class Sequence:
                  "repetition_penalty", "computed_token_num", "scheduled_token_num", "is_abort",
                  "mm_contents", "page_hashes", "num_cached_tokens", "arrival_time", "first_token_time",
                  "finish_time", "slot", "mrope_delta", "mm_state", "pt_np", "pending", "zombie", "pt_gen", "published",
-                 "slot_fresh", "logprobs", "output_logprobs")
+                 "slot_fresh", "logprobs", "output_logprobs", "seed", "frequency_penalty", "presence_penalty",
+                 "logit_bias")
 
     def __init__(self, seq_id: int, token_ids: List[int], finish_tokens: List[int],
                  output_len: Optional[int] = None, ignore_eos: bool = False, temperature: float = 0.6,
                  top_p: float = 0.9, top_k: int = 10, repetition_penalty: float = 1.0, mm_contents=None,
-                 logprobs: int = -1):
+                 logprobs: int = -1, seed: Optional[int] = None, frequency_penalty: float = 0.0,
+                 presence_penalty: float = 0.0, logit_bias: Optional[Dict[int, float]] = None):
         self.seq_id = seq_id
         self.token_ids: List[int] = list(token_ids)
         self.prompt_len = len(self.token_ids)
@@ -35,6 +37,13 @@ class Sequence:
         # (sampled token's log-prob, [(token, log-prob), ...]) per generated token, filled by the front-end
         self.logprobs = logprobs
         self.output_logprobs: list = []
+        # OpenAI sampling parameters: a seeded request draws from a stream keyed by (seed, token position), so its
+        # tokens depend on its logits alone; the penalties and logit_bias form an additive row on the device
+        # (`has_bias_row`), subtracted per generated occurrence / added per token id before the temperature
+        self.seed = seed
+        self.frequency_penalty = frequency_penalty
+        self.presence_penalty = presence_penalty
+        self.logit_bias = logit_bias or None
         # computed_token_num : tokens whose KV is computed AND whose batch has returned
         # scheduled_token_num: tokens covered by chunks scheduled so far (returned or in flight);
         #                      with pp_size > 1 several chunks of one prompt can be in flight
@@ -56,6 +65,10 @@ class Sequence:
         self.pending = -1    # index of a placeholder token reserved by a lookahead step (async scheduling)
         self.zombie = False  # finished while a lookahead step was already in flight: pages freed when it returns
         self.mm_state = None
+
+    @property
+    def has_bias_row(self) -> bool:
+        return self.frequency_penalty != 0.0 or self.presence_penalty != 0.0 or bool(self.logit_bias)
 
     def __len__(self):
         return len(self.token_ids)
