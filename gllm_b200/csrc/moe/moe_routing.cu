@@ -77,7 +77,7 @@ __global__ void topk_softmax_kernel(const __nv_bfloat16* __restrict__ logits, in
 }
 
 // ---------------------------------------------------------------------------------------------
-// grouped top-k (DeepSeek): one warp per token, E <= 512, groups <= 32
+// grouped top-k (DeepSeek): one warp per token, E <= 512, groups <= 32, any E % n_group == 0
 // ---------------------------------------------------------------------------------------------
 template <int VPT>
 __global__ void grouped_topk_kernel(const __nv_bfloat16* __restrict__ logits, int64_t ld, const float* __restrict__ bias,
@@ -87,7 +87,7 @@ __global__ void grouped_topk_kernel(const __nv_bfloat16* __restrict__ logits, in
   const int lane = threadIdx.x & 31;
   if (warp >= T) return;
   const __nv_bfloat16* row = logits + static_cast<size_t>(warp) * ld;
-  // expert e = lane * VPT + i  (contiguous per lane so a group maps to whole lanes when E/n_group >= VPT)
+  // expert e = lane * VPT + i
   float sc[VPT], sel[VPT];
   float mx = -INFINITY;
 #pragma unroll
@@ -115,29 +115,39 @@ __global__ void grouped_topk_kernel(const __nv_bfloat16* __restrict__ logits, in
     const int e = lane * VPT + i;
     sel[i] = e < E ? sc[i] + (bias != nullptr ? bias[e] : 0.f) : -INFINITY;
   }
-  // group score: sum of top-2 (bias-corrected) or max; lanes_per_group lanes cooperate
+  // group score: sum of the top-2 keys (bias-corrected) or the max key. A group need not fall on whole lanes
+  // (E = 160, 8 groups: 20 experts per group, 8 per lane), so for every group each lane takes the top-2 of its own
+  // experts of that group and a full-warp butterfly merges them; lane g keeps the score of group g.
   const int epg = E / n_group;            // experts per group
-  const int lpg = max(1, epg / VPT);      // lanes per group (epg multiple of VPT or lpg == 1)
-  float t1 = -INFINITY, t2 = -INFINITY;
+  int grp[VPT];                           // group of each of my experts (-1: padding)
 #pragma unroll
-  for (int i = 0; i < VPT; ++i) {
-    if (sel[i] > t1) { t2 = t1; t1 = sel[i]; } else if (sel[i] > t2) { t2 = sel[i]; }
+  for (int i = 0; i < VPT; ++i) grp[i] = lane * VPT + i < E ? (lane * VPT + i) / epg : -1;
+  float my_gscore = -INFINITY;
+  for (int g = 0; g < n_group; ++g) {
+    float t1 = -INFINITY, t2 = -INFINITY;
+#pragma unroll
+    for (int i = 0; i < VPT; ++i) {
+      if (grp[i] == g) {
+        if (sel[i] > t1) { t2 = t1; t1 = sel[i]; } else if (sel[i] > t2) { t2 = sel[i]; }
+      }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const float o1 = __shfl_xor_sync(0xffffffffu, t1, o), o2 = __shfl_xor_sync(0xffffffffu, t2, o);
+      if (o1 > t1) { t2 = fmaxf(t1, o2); t1 = o1; } else { t2 = fmaxf(t2, o1); }
+    }
+    if (lane == g) my_gscore = (bias != nullptr) ? t1 + t2 : t1;
   }
-  for (int o = 1; o < lpg; o <<= 1) {
-    const float o1 = __shfl_xor_sync(0xffffffffu, t1, o), o2 = __shfl_xor_sync(0xffffffffu, t2, o);
-    if (o1 > t1) { t2 = fmaxf(t1, o2); t1 = o1; } else { t2 = fmaxf(t2, o1); }
-  }
-  float gscore = (bias != nullptr) ? t1 + t2 : t1;
-  const int my_group = (lane * VPT) / epg;
-  // rank of my group among groups: count groups with a strictly better score (ties: lower index wins)
+  // lane g < n_group: rank of group g = number of groups with a strictly better score (ties: lower index wins)
   int better = 0;
   for (int g = 0; g < n_group; ++g) {
-    const float gs = __shfl_sync(0xffffffffu, gscore, (g * epg) / VPT);
-    if (gs > gscore || (gs == gscore && g < my_group)) ++better;
+    const float gs = __shfl_sync(0xffffffffu, my_gscore, g);
+    if (gs > my_gscore || (gs == my_gscore && g < lane)) ++better;
   }
-  const bool group_on = (lane * VPT < E) && better < topk_group;
+  const unsigned group_on = __ballot_sync(0xffffffffu, lane < n_group && better < topk_group);
+  // the group mask applies per expert
 #pragma unroll
-  for (int i = 0; i < VPT; ++i) if (!group_on) sel[i] = -INFINITY;
+  for (int i = 0; i < VPT; ++i) if (grp[i] < 0 || !((group_on >> grp[i]) & 1u)) sel[i] = -INFINITY;
   float wsum = 0.f, my_w = 0.f;
   int my_id = 0;
   for (int k = 0; k < K; ++k) {
@@ -254,7 +264,11 @@ using namespace b200;
 GLLM_EXPORT int gllm_moe_topk_softmax(const void* logits, int64_t ld, void* w_out, void* id_out, int T, int E, int K,
                                       int renorm, void* stream) {
   if (T <= 0) return 0;
-  if (E > 512 || K > 32) { fprintf(stderr, "[gllm_b200] topk_softmax: E<=512, K<=32 only\n"); return 1; }
+  // K > E would return padding ids >= E (they index expert_map next)
+  if (E < 1 || E > 512 || K < 1 || K > 32 || K > E) {
+    fprintf(stderr, "[gllm_b200] topk_softmax: unsupported E=%d K=%d (1 <= K <= min(E, 32), E <= 512)\n", E, K);
+    return 1;
+  }
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const int blocks = (T * 32 + 255) / 256;
   auto L = reinterpret_cast<const __nv_bfloat16*>(logits);
@@ -275,10 +289,12 @@ GLLM_EXPORT int gllm_moe_grouped_topk(const void* logits, int64_t ld, const void
                                       float scaling, void* stream) {
   if (T <= 0) return 0;
   const int vpt = (E + 31) / 32;
-  const int epg = E / n_group;
-  if (E > 512 || K > 32 || E % n_group != 0 || (epg % vpt != 0 && epg > vpt) || (epg < vpt && vpt % epg != 0) ||
-      epg < vpt) {
-    fprintf(stderr, "[gllm_b200] grouped_topk: unsupported E=%d groups=%d\n", E, n_group);
+  // one warp per token: E <= 512; group scores live one per lane: n_group <= 32; the K winners must come from the
+  // experts of the topk_group best groups, else the kernel would return padding ids >= E
+  if (E < 1 || E > 512 || K < 1 || K > 32 || K > E || n_group < 1 || n_group > 32 || E % n_group != 0 ||
+      topk_group < 1 || K > min(topk_group, n_group) * (E / n_group)) {
+    fprintf(stderr, "[gllm_b200] grouped_topk: unsupported E=%d K=%d groups=%d topk_group=%d\n", E, K, n_group,
+            topk_group);
     return 1;
   }
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
@@ -305,6 +321,13 @@ GLLM_EXPORT int gllm_moe_align_gather(const void* ids, const void* expert_map, i
                                       int64_t ldx, void* xs, int H, const void* n_valid, void* stream) {
   const int n_slots = T * top_k;
   if (n_slots <= 0) return 0;
+  // moe_offsets_kernel keeps the offsets in a fixed shared array; the gather copies rows in 16-byte pieces
+  if (E_local < 1 || E_local > 1024 || H % 8 != 0 || ldx % 8 != 0 || reinterpret_cast<uintptr_t>(x) % 16 != 0 ||
+      reinterpret_cast<uintptr_t>(xs) % 16 != 0) {
+    fprintf(stderr, "[gllm_b200] moe_align_gather: unsupported E_local=%d H=%d ldx=%lld or misaligned x / xs\n",
+            E_local, H, static_cast<long long>(ldx));
+    return 1;
+  }
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   CUDA_CHECK_RET(cudaMemsetAsync(meta, 0, sizeof(int32_t) * (2 + 3 * E_local + 1), st));
   moe_count_kernel<<<(n_slots + 255) / 256, 256, 0, st>>>(reinterpret_cast<const int32_t*>(ids),
