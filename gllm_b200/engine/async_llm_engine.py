@@ -76,6 +76,7 @@ class AsyncStream:
         self.first_token_time: Optional[float] = None
         self.seq_id = -1
         self.aborted = False     # an abort id was sent for this request (front-end side state only)
+        self.group: Optional[list] = None   # parallel sampling: the streams of all choices of the request
 
     def put(self, item: str):
         """Queue a text delta. With stop strings (OpenAI `stop`; not honoured by the reference) the text that could
@@ -182,22 +183,31 @@ class AsyncLLM(LLM):
     async def add_requests_async(self, raw_request, token_ids: List[int], output_len=None, ignore_eos=False,
                                  temperature=None, top_p=None, top_k=None, repetition_penalty=None,
                                  mm_contents=None, stop=None, logprobs=None, seed=None, frequency_penalty=None,
-                                 presence_penalty=None, logit_bias=None) -> AsyncStream:
+                                 presence_penalty=None, logit_bias=None, n=None):
         """`logprobs`: None, or N in [0, 20] — every text delta of the stream is then a `Delta` carrying the
         log-prob entries of the tokens whose text it releases (see `LLM.generate`). `seed`, `frequency_penalty`,
-        `presence_penalty`, `logit_bias`: see `LLM.allocate_seq` (ValueError when out of range)."""
-        seq = self.allocate_seq(token_ids, output_len, ignore_eos, temperature, top_p, top_k, repetition_penalty,
-                                mm_contents, logprobs, seed, frequency_penalty, presence_penalty, logit_bias)
-        stream = AsyncStream(raw_request, stop, logprobs=logprobs is not None)
-        stream.prompt_tokens = len(token_ids)
-        stream.seq_id = seq.seq_id
-        self.async_streams[seq.seq_id] = stream
-        self.metrics["requests_total"] += 1
+        `presence_penalty`, `logit_bias`: see `LLM.allocate_seq` (ValueError when out of range).
+        Returns the request's `AsyncStream`; with `n` given (parallel sampling, see `LLM.allocate_choices`) a list of
+        one stream per choice, in choice order. A stop string ends only its own choice."""
+        seqs = self.allocate_choices(token_ids, n, output_len, ignore_eos, temperature, top_p, top_k,
+                                     repetition_penalty, mm_contents, logprobs, seed, frequency_penalty,
+                                     presence_penalty, logit_bias)
+        streams = []
+        for seq in seqs:
+            stream = AsyncStream(raw_request, stop, logprobs=logprobs is not None)
+            stream.prompt_tokens = len(token_ids)
+            stream.seq_id = seq.seq_id
+            self.async_streams[seq.seq_id] = stream
+            streams.append(stream)
+        if len(streams) > 1:
+            for st in streams:
+                st.group = streams
+        self.metrics["requests_total"] += 1          # requests, not choices
         self.metrics["prompt_tokens_total"] += len(token_ids)
-        self.add_requests([seq])
+        self.add_requests(seqs[:1])
         if self._task is None and self.failed is None:
             self.start_schedule_engine()
-        return stream
+        return streams if n is not None else streams[0]
 
     def abort_stream(self, stream: AsyncStream):
         """Client went away: abort the request so its KV pages are freed (reference:
@@ -206,9 +216,11 @@ class AsyncLLM(LLM):
         # Only the abort id is sent: the Sequence object is shared with the in-proc scheduler, which must be the
         # one to take it out of its queues before flagging it (a flag set from here while a prefill chunk was in
         # flight left a freed sequence at the head of the prefill queue and took the engine down).
-        if not stream.aborted and not stream.finished:
-            stream.aborted = True
-            self.abort([stream.seq_id])
+        live = [st for st in (stream.group or [stream]) if not st.aborted and not st.finished]
+        if live:           # every choice of the request
+            for st in live:
+                st.aborted = True
+            self.abort([st.seq_id for st in live])
             self.metrics["requests_aborted"] += 1
 
     async def collect(self, stream: AsyncStream) -> str:
@@ -244,9 +256,10 @@ class AsyncLLM(LLM):
                 continue
             if st.first_token_time is None:
                 st.first_token_time = time.time()
-                self.metrics["ttft_sum"] += st.first_token_time - st.created
-                self.metrics["ttft_count"] += 1
-                self.hist["ttft"].observe(st.first_token_time - st.created)
+                if st.group is None or all(o.first_token_time is None for o in st.group if o is not st):
+                    self.metrics["ttft_sum"] += st.first_token_time - st.created     # once per request
+                    self.metrics["ttft_count"] += 1
+                    self.hist["ttft"].observe(st.first_token_time - st.created)
             st.completion_tokens = seq.num_output_tokens
             if st.want_logprobs:
                 self._deliver_with_logprobs(seq, st)
@@ -288,9 +301,11 @@ class AsyncLLM(LLM):
             if st is not None:
                 st.completion_tokens = seq.num_output_tokens
                 self.metrics["generation_tokens_total"] += seq.num_output_tokens
-                self.metrics["requests_finished"] += 1
                 now = time.time()
-                self.hist["e2e"].observe(now - st.created)
+                # a request with several choices counts once, when its last choice ends
+                if st.group is None or all(o.finished for o in st.group if o is not st):
+                    self.metrics["requests_finished"] += 1
+                    self.hist["e2e"].observe(now - st.created)
                 if st.first_token_time is not None and seq.num_output_tokens > 1:
                     self.hist["tpot"].observe((now - st.first_token_time) / (seq.num_output_tokens - 1))
                 reason = "length" if seq.num_output_tokens >= seq.output_len else "stop"

@@ -33,6 +33,30 @@ from gllm_b200.sequence import Sequence
 MAX_LOGPROBS = 20   # most likely tokens reported per generated token (csrc/sample/sampler.cu: kMaxLogprobs)
 # logit_bias entries per request: this engine's own cap (one scatter per entry when the bias row is rebuilt)
 MAX_LOGIT_BIAS = 1024
+MAX_N = 128         # choices per request (parallel sampling, OpenAI `n`)
+
+
+def check_n(n, max_running_seqs: int, multimodal: bool = False) -> int:
+    """Validate OpenAI `n` -> the number of choices. None means 1. Raises ValueError: n must be an integer in
+    [1, MAX_N] and at most the engine's max_running_seqs (all first tokens are drawn in one batch); n > 1 with
+    multimodal input is not supported."""
+    if n is None:
+        return 1
+    if isinstance(n, bool) or not isinstance(n, int) and not (isinstance(n, float) and n.is_integer()):
+        raise ValueError("n must be an integer")
+    n = int(n)
+    if not 1 <= n <= min(MAX_N, max_running_seqs):
+        raise ValueError(f"n must be in [1, {min(MAX_N, max_running_seqs)}]")
+    if n > 1 and multimodal:
+        raise ValueError("n > 1 is not supported with multimodal input")
+    return n
+
+
+def choice_seed(seed: Optional[int], i: int) -> Optional[int]:
+    """Seed of choice i of a request seeded with `seed`: seed + i, wrapped to a signed 64-bit int."""
+    if seed is None:
+        return None
+    return (seed + i + 2 ** 63) % 2 ** 64 - 2 ** 63
 
 
 def check_sampling_params(seed=None, frequency_penalty=None, presence_penalty=None, logit_bias=None,
@@ -285,6 +309,29 @@ class LLM:
         seq.arrival_time = time.time()
         return seq
 
+    def allocate_choices(self, token_ids: List[int], n=None, output_len=None, ignore_eos=False, temperature=None,
+                         top_p=None, top_k=None, repetition_penalty=None, mm_contents=None, logprobs=None, seed=None,
+                         frequency_penalty=None, presence_penalty=None, logit_bias=None) -> List[Sequence]:
+        """The `n` choices of one request (parallel sampling; see `check_n`): choice 0 is the request as `allocate_seq`
+        makes it, choices 1..n-1 are its forks (`Sequence.forks`): the prompt is prefilled once and every choice draws
+        its first token from the same logits row, then continues on its own. With a seed, choice i uses seed + i.
+        Only choice 0 goes to `add_requests`; the forks travel with it."""
+        k = check_n(n, self.cfg.max_running_seqs, bool(mm_contents))
+        seqs = []
+        try:
+            for i in range(k):
+                seqs.append(self.allocate_seq(token_ids, output_len, ignore_eos, temperature, top_p, top_k,
+                                              repetition_penalty, mm_contents, logprobs,
+                                              choice_seed(seed, i) if i else seed, frequency_penalty, presence_penalty,
+                                              logit_bias))
+        except Exception:
+            with self._inbox_lock:
+                for s in seqs:
+                    self.id_allocator.free(s.seq_id)
+            raise
+        seqs[0].forks = seqs[1:]
+        return seqs
+
     # The three inboxes below are filled from request handlers (event-loop thread of the API server) while the
     # engine tick runs in a worker thread: every append and the swap in `_send` hold `_inbox_lock`, so a request
     # can never land in a list the tick has already shipped (the reference has this race, SURVEY §5.2).
@@ -308,6 +355,8 @@ class LLM:
             cmds, self.control_cmds = self.control_cmds, []
         for seq in wait:
             self.running_maps[seq.seq_id] = seq
+            for sib in seq.forks:
+                self.running_maps[sib.seq_id] = sib
         if cmds:
             for cmd in cmds[:-1]:
                 self._post(IPCPackage(control_cmd=cmd))
@@ -375,7 +424,7 @@ class LLM:
                  output_lens: Optional[List[int]] = None, temperature=None, top_p=None, top_k=None,
                  repetition_penalty=None, ignore_eos: bool = False, progress: bool = False,
                  mm_contents: Optional[List[Optional[dict]]] = None, logprobs=None, seed=None,
-                 frequency_penalty=None, presence_penalty=None, logit_bias=None) -> List[Sequence]:
+                 frequency_penalty=None, presence_penalty=None, logit_bias=None, n=None) -> List[Sequence]:
         """Batch generation; returns the finished `Sequence`s in request order with `.prompt`,
         `.output`, `.token_ids` (reference: gllm/llm_engine.py:343-378). `mm_contents[i]` (VL models) is
         the processor output of request i: pixel_values / image_grid_thw [/ pixel_values_videos ...].
@@ -383,14 +432,15 @@ class LLM:
         (its log-prob, [(token, log-prob) of the N most likely tokens]) in `.output_logprobs`, under the raw model
         distribution (log_softmax of the logits, before penalty / temperature / top-k / top-p).
         `seed`, `frequency_penalty`, `presence_penalty`, `logit_bias` ({token id: bias}): OpenAI sampling parameters,
-        one value or one per request like the others (a dict is one value for all requests)."""
+        one value or one per request like the others (a dict is one value for all requests).
+        `n` (parallel sampling, one value or one per request): request j gives n_j choices, returned consecutively in
+        choice order; the prompt is prefilled once (see `allocate_choices`)."""
         if self.worker is not None and self.worker.rank != 0:
             return self._serve_until_stop()
         if tokens is None:
             assert prompts is not None
             tokens = [self.encode(p) for p in prompts]
-        n = len(tokens)
-        seqs = []
+        seqs, heads = [], []
         for i, toks in enumerate(tokens):
             ol = output_lens[i] if output_lens is not None else None
             if not self.check_seq_length(toks, ol):
@@ -398,12 +448,15 @@ class LLM:
                                  f"{self.model_max_length}")
             def pick(v):            # sampling parameters: one value for all requests, or one per request
                 return v[i] if isinstance(v, (list, tuple)) else v
-            seqs.append(self.allocate_seq(toks, ol, ignore_eos, pick(temperature), pick(top_p), pick(top_k),
-                                          pick(repetition_penalty),
-                                          mm_contents[i] if mm_contents is not None else None, pick(logprobs),
-                                          pick(seed), pick(frequency_penalty), pick(presence_penalty),
-                                          pick(logit_bias)))
-        self.add_requests(seqs)
+            choices = self.allocate_choices(toks, pick(n), ol, ignore_eos, pick(temperature), pick(top_p), pick(top_k),
+                                            pick(repetition_penalty),
+                                            mm_contents[i] if mm_contents is not None else None, pick(logprobs),
+                                            pick(seed), pick(frequency_penalty), pick(presence_penalty),
+                                            pick(logit_bias))
+            heads.append(choices[0])
+            seqs.extend(choices)
+        n = len(seqs)
+        self.add_requests(heads)
         base = len(self.finished)
         bar = None
         if progress:

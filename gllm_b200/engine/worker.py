@@ -104,9 +104,10 @@ class Worker(ProfilerMixin):
         for pkg in pkgs:
             if pkg.schedule_lists:
                 for seq in pkg.schedule_lists:
-                    seq.slot = 0        # penalty state rows are assigned at the first emission (`_assign_slots`)
-                    if seq.repetition_penalty != 1.0 or seq.has_bias_row:
-                        self._penalty_seen = True
+                    for s in [seq] + seq.forks:
+                        s.slot = 0      # penalty state rows are assigned at the first emission (`_assign_slots`)
+                        if s.repetition_penalty != 1.0 or s.has_bias_row:
+                            self._penalty_seen = True
                 self.scheduler.add_new_requests(pkg.schedule_lists)
             if pkg.abort_ids:
                 self.scheduler.add_abort_ids(pkg.abort_ids)
@@ -182,15 +183,17 @@ class Worker(ProfilerMixin):
         if not self._penalty_seen:
             return          # no request with a penalty or logit_bias has arrived yet: nothing to scan per step
         for e in entries:
-            seq = e.seq
-            if e.emits and (seq.repetition_penalty != 1.0 or seq.has_bias_row) and seq.slot <= 0:
-                if self._free_slots:
-                    seq.slot = self._free_slots.pop()
-                else:
-                    seq.slot = self._num_slots
-                    self._num_slots += 1
-                seq.slot_fresh = True
-                self._seq_slots[seq.seq_id] = seq.slot
+            if not e.emits:
+                continue
+            for seq in [e.seq] + (e.forks or []):     # (forks: the other choices of a fan-out, first emission)
+                if (seq.repetition_penalty != 1.0 or seq.has_bias_row) and seq.slot <= 0:
+                    if self._free_slots:
+                        seq.slot = self._free_slots.pop()
+                    else:
+                        seq.slot = self._num_slots
+                        self._num_slots += 1
+                    seq.slot_fresh = True
+                    self._seq_slots[seq.seq_id] = seq.slot
 
     def _release_slot(self, seq):
         slot = self._seq_slots.pop(seq.seq_id, 0)

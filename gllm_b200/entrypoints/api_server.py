@@ -61,15 +61,20 @@ def _validate_logprobs(request, chat: bool):
     return None
 
 
-def _check_params(request):
-    """-> (error message or None, kwargs of the OpenAI sampling parameters for add_requests_async)."""
-    from gllm_b200.engine.llm_engine import check_sampling_params
+def _check_params(request, multimodal: bool = False):
+    """-> (error message or None, kwargs of the OpenAI sampling parameters for add_requests_async). `n` is passed
+    only when it is above 1, so an n = 1 request takes exactly the path it took before parallel sampling."""
+    from gllm_b200.engine.llm_engine import check_n, check_sampling_params
     try:
         seed, f, p, lb = check_sampling_params(request.seed, request.frequency_penalty, request.presence_penalty,
                                                request.logit_bias, llm.loader.config.get("vocab_size"))
+        n = check_n(request.n, llm.cfg.max_running_seqs, multimodal)
     except (ValueError, TypeError) as e:
         return str(e), None
-    return None, dict(seed=seed, frequency_penalty=f, presence_penalty=p, logit_bias=lb)
+    out = dict(seed=seed, frequency_penalty=f, presence_penalty=p, logit_bias=lb)
+    if n > 1:
+        out["n"] = n
+    return None, out
 
 
 def _token_str(tok: int) -> str:
@@ -116,79 +121,121 @@ def _validate(token_ids, output_len, vocab_size=None):
     return None
 
 
-def _usage(stream) -> UsageInfo:
-    return UsageInfo(prompt_tokens=stream.prompt_tokens, completion_tokens=stream.completion_tokens,
-                     total_tokens=stream.prompt_tokens + stream.completion_tokens)
+def _usage(streams) -> UsageInfo:
+    """The prompt counts once; the completion tokens of every choice (parallel sampling) add up."""
+    done = sum(st.completion_tokens for st in streams)
+    return UsageInfo(prompt_tokens=streams[0].prompt_tokens, completion_tokens=done,
+                     total_tokens=streams[0].prompt_tokens + done)
+
+
+async def _merge(streams):
+    """Interleave the deltas of the choices' streams as they come: yields (choice index, delta), and
+    (choice index, None) when that choice has ended."""
+    q: asyncio.Queue = asyncio.Queue()
+
+    async def pump(i, st):
+        try:
+            async for d in st:
+                await q.put((i, d))
+        except Exception as e:  # noqa: BLE001 (engine failure: re-raised in the consumer)
+            await q.put((i, e))
+            return
+        await q.put((i, None))
+    tasks = [asyncio.get_running_loop().create_task(pump(i, st)) for i, st in enumerate(streams)]
+    left = len(streams)
+    try:
+        while left:
+            i, d = await q.get()
+            if isinstance(d, Exception):
+                raise d
+            if d is None:
+                left -= 1
+            yield i, d
+    finally:
+        for t in tasks:
+            t.cancel()
 
 
 # ------------------------------------------------------------------------------------------------
 # response generators (reference: serving_chat.py / serving_completions.py)
 # ------------------------------------------------------------------------------------------------
-async def chat_completion_generator(stream, request) -> ChatCompletionResponse:
-    text = await llm.collect(stream)
-    choice = ChatCompletionResponseChoice(index=0, message=ChatMessage(role="assistant", content=text),
-                                          finish_reason=stream.finish_reason)
-    if stream.want_logprobs:
-        choice.logprobs = _chat_logprobs(stream.logprobs_out)
-    return ChatCompletionResponse(choices=[choice], usage=_usage(stream), model=request.model)
+async def chat_completion_generator(streams, request) -> ChatCompletionResponse:
+    texts = await asyncio.gather(*(llm.collect(st) for st in streams))
+    choices = []
+    for i, (st, text) in enumerate(zip(streams, texts)):
+        choice = ChatCompletionResponseChoice(index=i, message=ChatMessage(role="assistant", content=text),
+                                              finish_reason=st.finish_reason)
+        if st.want_logprobs:
+            choice.logprobs = _chat_logprobs(st.logprobs_out)
+        choices.append(choice)
+    return ChatCompletionResponse(choices=choices, usage=_usage(streams), model=request.model)
 
 
-async def chat_completion_stream_generator(stream, request):
+async def chat_completion_stream_generator(streams, request):
+    """`streams`: one per choice. One choice per chunk, with its index; every choice ends with its own finish chunk,
+    and the last of those carries the usage of the whole request (with one choice: today's single-choice stream)."""
     rid = None
-    first = True
+    first = [True] * len(streams)
+    left = len(streams)
     try:
-        async for delta in stream:
-            dm = DeltaMessage(role="assistant", content=delta) if first else DeltaMessage(content=delta)
-            first = False
-            chunk = ChatCompletionStreamResponse(
-                choices=[ChatCompletionResponseStreamChoice(index=0, delta=dm)], model=request.model)
-            if stream.want_logprobs:
-                chunk.choices[0].logprobs = _chat_logprobs(delta.logprobs)
+        async for i, delta in _merge(streams):
+            st = streams[i]
+            if delta is None:
+                left -= 1
+                chunk = ChatCompletionStreamResponse(
+                    choices=[ChatCompletionResponseStreamChoice(index=i, delta=DeltaMessage(),
+                                                                finish_reason=st.finish_reason or "stop")],
+                    model=request.model, usage=_usage(streams) if left == 0 else None)
+            else:
+                dm = DeltaMessage(role="assistant", content=delta) if first[i] else DeltaMessage(content=delta)
+                first[i] = False
+                chunk = ChatCompletionStreamResponse(
+                    choices=[ChatCompletionResponseStreamChoice(index=i, delta=dm)], model=request.model)
+                if st.want_logprobs:
+                    chunk.choices[0].logprobs = _chat_logprobs(delta.logprobs)
             if rid is None:
                 rid = chunk.id
             chunk.id = rid
             yield f"data: {chunk.model_dump_json(exclude_none=True)}\n\n"
     finally:
-        llm.abort_stream(stream)  # no-op unless the client disconnected mid-stream
-    final = ChatCompletionStreamResponse(
-        choices=[ChatCompletionResponseStreamChoice(index=0, delta=DeltaMessage(),
-                                                    finish_reason=stream.finish_reason or "stop")],
-        model=request.model, usage=_usage(stream))
-    if rid is not None:
-        final.id = rid
-    yield f"data: {final.model_dump_json(exclude_none=True)}\n\n"
+        llm.abort_stream(streams[0])  # every choice; no-op unless the client disconnected mid-stream
     yield "data: [DONE]\n\n"
 
 
-async def completion_generator(stream, request) -> CompletionResponse:
-    text = await llm.collect(stream)
-    choice = CompletionResponseChoice(index=0, text=text, finish_reason=stream.finish_reason)
-    if stream.want_logprobs:
-        choice.logprobs = _completion_logprobs(stream.logprobs_out)[0]
-    return CompletionResponse(choices=[choice], model=request.model, usage=_usage(stream))
+async def completion_generator(streams, request) -> CompletionResponse:
+    texts = await asyncio.gather(*(llm.collect(st) for st in streams))
+    choices = []
+    for i, (st, text) in enumerate(zip(streams, texts)):
+        choice = CompletionResponseChoice(index=i, text=text, finish_reason=st.finish_reason)
+        if st.want_logprobs:
+            choice.logprobs = _completion_logprobs(st.logprobs_out)[0]
+        choices.append(choice)
+    return CompletionResponse(choices=choices, model=request.model, usage=_usage(streams))
 
 
-async def completion_stream_generator(stream, request):
+async def completion_stream_generator(streams, request):
     rid = None
-    offset = 0
+    offset = [0] * len(streams)
+    left = len(streams)
     try:
-        async for delta in stream:
-            chunk = CompletionStreamResponse(choices=[CompletionResponseStreamChoice(index=0, text=delta)],
-                                             model=request.model)
-            if stream.want_logprobs:
-                chunk.choices[0].logprobs, offset = _completion_logprobs(delta.logprobs, offset)
+        async for i, delta in _merge(streams):
+            st = streams[i]
+            if delta is None:
+                left -= 1
+                chunk = CompletionStreamResponse(
+                    choices=[CompletionResponseStreamChoice(index=i, text="", finish_reason=st.finish_reason or "stop")],
+                    model=request.model, usage=_usage(streams) if left == 0 else None)
+            else:
+                chunk = CompletionStreamResponse(choices=[CompletionResponseStreamChoice(index=i, text=delta)],
+                                                 model=request.model)
+                if st.want_logprobs:
+                    chunk.choices[0].logprobs, offset[i] = _completion_logprobs(delta.logprobs, offset[i])
             if rid is None:
                 rid = chunk.id
             chunk.id = rid
             yield f"data: {chunk.model_dump_json(exclude_unset=False)}\n\n"
     finally:
-        llm.abort_stream(stream)  # no-op unless the client disconnected mid-stream
-    final = CompletionStreamResponse(
-        choices=[CompletionResponseStreamChoice(index=0, text="", finish_reason=stream.finish_reason or "stop")],
-        model=request.model, usage=_usage(stream))
-    if rid is not None:
-        final.id = rid
-    yield f"data: {final.model_dump_json(exclude_unset=False)}\n\n"
+        llm.abort_stream(streams[0])  # every choice; no-op unless the client disconnected mid-stream
     yield "data: [DONE]\n\n"
 
 
@@ -266,7 +313,7 @@ def build_app(engine):
                 token_ids = await _in_thread(llm.encode, None, True, request.messages)
         except Exception as e:  # noqa: BLE001
             return _error(f"cannot encode messages: {e}")
-        bad, params = _check_params(request)
+        bad, params = _check_params(request, multimodal=bool(mm_contents))
         bad = bad or _validate_sampling(request) or _validate_logprobs(request, chat=True) or \
             _validate(token_ids, request.output_len(), llm.loader.config.get("vocab_size"))
         if bad:
@@ -278,10 +325,11 @@ def build_app(engine):
                                               request.repetition_penalty, mm_contents, stop=request.stop,
                                               logprobs=(request.top_logprobs or 0) if request.logprobs else None,
                                               **params)
+        streams = stream if "n" in params else [stream]
         if request.stream:
-            return StreamingResponse(chat_completion_stream_generator(stream, request),
+            return StreamingResponse(chat_completion_stream_generator(streams, request),
                                      media_type="text/event-stream")
-        return JSONResponse(content=(await chat_completion_generator(stream, request)).model_dump())
+        return JSONResponse(content=(await chat_completion_generator(streams, request)).model_dump())
 
     @app.post("/v1/completions")
     async def create_completion(request: CompletionRequest, raw_request: Request):
@@ -300,9 +348,10 @@ def build_app(engine):
                                               request.temperature, request.top_p, request.top_k,
                                               request.repetition_penalty, stop=request.stop,
                                               logprobs=request.logprobs, **params)
+        streams = stream if "n" in params else [stream]
         if request.stream:
-            return StreamingResponse(completion_stream_generator(stream, request), media_type="text/event-stream")
-        return JSONResponse(content=(await completion_generator(stream, request)).model_dump())
+            return StreamingResponse(completion_stream_generator(streams, request), media_type="text/event-stream")
+        return JSONResponse(content=(await completion_generator(streams, request)).model_dump())
 
     @app.post("/tokenize")
     async def tokenize(request: TokenizeRequest):

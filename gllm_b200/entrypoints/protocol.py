@@ -27,6 +27,16 @@ it draws the same token whatever the batch, its row in it, the engine's step cou
 or the tensor-parallel degree; without a seed the draw comes from the engine's own stream. A 400 answers: a penalty
 outside [-2, 2] or not finite; a logit_bias key that is not an int in [0, vocab_size), a value outside [-100, 100] or
 not finite, or more than 1024 entries (this engine's own cap); a seed that does not fit a signed 64-bit int.
+
+`n` asks for n independent choices of one request (parallel sampling). The prompt is prefilled once, its full KV
+pages are shared by the choices and its partial last page is copied on the device; every choice draws its first token
+from the same logits row, then continues as a sequence of its own with its own stop handling, `finish_reason` and
+logprobs. `choices[i].index` is i. `usage.prompt_tokens` counts the prompt once, `completion_tokens` is summed over the
+choices. When streaming, every chunk carries one choice with its index, each choice ends with its own finish chunk and
+the last finish chunk carries `usage`. With `seed = s`, choice i draws as an n = 1 request seeded with s + i would
+(wrapping in signed 64-bit). A stop string ends only its own choice; a client disconnect aborts all of them. `n` must
+be an integer in [1, 128] and at most the engine's max_running_seqs, and n > 1 is refused with multimodal input (400).
+`n = 1` (or absent) gives exactly the single-choice response. `best_of` is ignored.
 """
 from __future__ import annotations
 

@@ -78,6 +78,9 @@ class BatchArrays:
     # seeded rows (None when no row has a seed): request seed and position of the token being produced (-1: unseeded)
     seed: Optional[np.ndarray] = None        # int64 [E]
     seed_pos: Optional[np.ndarray] = None    # int32 [E]
+    # parallel sampling: (src, dst) KV pages every rank copies for its own layers right after this batch's forward
+    # (the partial last prompt page of a request that fans out into several choices); None when there is none
+    kv_copy: Optional[np.ndarray] = None     # int32 [C, 2]
     emit_ids: Optional[list] = None  # driver-local: sequence id per EMITTING entry (order of the sampler output)
     seq_ids: Optional[list] = None  # driver-local: sequence id per row (incremental decode batches); not sent
     pt_gens: Optional[list] = None  # driver-local: Sequence.pt_gen per row when the block table rows were written
@@ -93,7 +96,7 @@ class BatchArrays:
                  "logits_idx", "emit_seq", "temperature", "top_k", "top_p", "rep_penalty", "state_slot"]
         opt = ["seen_rows", "seen_tokens", "clear_slots", "feed_src", "logprobs_n", "freq_pen", "pres_pen",
                "bias_slot", "rb_slots", "rb_pen", "rb_lb_off", "rb_lb_ids", "rb_lb_vals", "rb_out_off", "rb_out_toks",
-               "seed", "seed_pos"]
+               "seed", "seed_pos", "kv_copy"]
         scalars = (self.num_decode_seqs, self.num_seqs, self.num_tokens, self.max_q_len, self.max_seq_len,
                    self.all_greedy, self.need_penalty, self.batch_id)
         if self.need_bias:      # (only then: a batch without the feature sends the header it always sent)
@@ -259,6 +262,7 @@ def build_batch(entries, page_size: int, vocab_size: int, batch_id: int = 0, mro
     freq_pen, pres_pen, bias_slot, need_bias = [], [], [], False
     rb_slots, rb_pen, rb_lb_ids, rb_lb_vals, rb_out_toks, rb_lb_off, rb_out_off = [], [], [], [], [], [0], [0]
     seeds, seed_pos, want_seed = [], [], False
+    emit_rows, fork_rows, kv_copy = [], [], []   # (entry, logits row, sequence, end of its known tokens)
     for i, e in enumerate(entries):
         seq = e.seq
         pt = _page_array(seq)
@@ -284,58 +288,67 @@ def build_batch(entries, page_size: int, vocab_size: int, batch_id: int = 0, mro
                 positions[a:z] = pos
             slots[a:z] = pt[pos // page_size] * page_size + pos % page_size
         if e.emits:
-            emit_seq.append(i)
-            logits_idx.append(z - 1)
-            temperature.append(seq.temperature)
-            k = seq.top_k
-            top_k.append(vocab_size if (k is None or k <= 0 or k > vocab_size) else k)
-            top_p.append(seq.top_p)
-            rep_pen.append(seq.repetition_penalty)
-            state_slot.append(seq.slot)
-            logprobs_n.append(seq.logprobs)
-            if seq.logprobs >= 0:
-                want_logprobs = True
-            if top_k[-1] != 1:
-                all_greedy = False
-            # the state row was just (re)assigned — first emission, or first one after a preemption: its contents are
-            # rebuilt from everything known so far
-            fresh = seq.slot_fresh
-            seq.slot_fresh = False
-            if seq.seed is not None:
-                want_seed = True
-                seeds.append(seq.seed)
-                seed_pos.append(s0 + e.n)          # index of the token this step produces
+            emit_rows.append((i, z - 1, seq, s0 + e.n))
+            for sib in e.forks or ():        # parallel sampling: the other choices draw from the same logits row
+                fork_rows.append((i, z - 1, sib, s0 + e.n))
+            if e.kv_copy:
+                kv_copy.extend(e.kv_copy)
+    emit_ids = []
+    for i, row, seq, end in emit_rows + fork_rows:
+        emit_seq.append(i)
+        emit_ids.append(seq.seq_id)
+        logits_idx.append(row)
+        temperature.append(seq.temperature)
+        k = seq.top_k
+        top_k.append(vocab_size if (k is None or k <= 0 or k > vocab_size) else k)
+        top_p.append(seq.top_p)
+        rep_pen.append(seq.repetition_penalty)
+        state_slot.append(seq.slot)
+        logprobs_n.append(seq.logprobs)
+        if seq.logprobs >= 0:
+            want_logprobs = True
+        if top_k[-1] != 1:
+            all_greedy = False
+        # the state row was just (re)assigned — first emission, or first one after a preemption: its contents are
+        # rebuilt from everything known so far
+        fresh = seq.slot_fresh
+        seq.slot_fresh = False
+        if seq.seed is not None:
+            want_seed = True
+            seeds.append(seq.seed)
+            seed_pos.append(end)               # index of the token this step produces
+        else:
+            seeds.append(0)
+            seed_pos.append(-1)
+        if seq.has_bias_row:
+            need_bias = True
+            bias_slot.append(seq.slot)
+            freq_pen.append(seq.frequency_penalty)
+            pres_pen.append(seq.presence_penalty)
+            if fresh:
+                rb_slots.append(seq.slot)
+                rb_pen.append((seq.frequency_penalty, seq.presence_penalty))
+                lb = seq.logit_bias or {}
+                rb_lb_ids.extend(lb.keys())
+                rb_lb_vals.extend(lb.values())
+                rb_lb_off.append(len(rb_lb_ids))
+                rb_out_toks.extend(seq.token_ids[seq.prompt_len:end])
+                rb_out_off.append(len(rb_out_toks))
+        else:
+            bias_slot.append(-1)
+            freq_pen.append(0.0)
+            pres_pen.append(0.0)
+        if seq.repetition_penalty != 1.0:
+            need_penalty = True
+            if fresh:
+                # everything known so far (prompt and the tokens generated before) becomes "seen"
+                clear_slots.append(seq.slot)
+                seen_rows.append(np.full(end, seq.slot, dtype=np.int32))
+                seen_tokens.append(np.asarray(seq.token_ids[:end], dtype=np.int32))
             else:
-                seeds.append(0)
-                seed_pos.append(-1)
-            if seq.has_bias_row:
-                need_bias = True
-                bias_slot.append(seq.slot)
-                freq_pen.append(seq.frequency_penalty)
-                pres_pen.append(seq.presence_penalty)
-                if fresh:
-                    rb_slots.append(seq.slot)
-                    rb_pen.append((seq.frequency_penalty, seq.presence_penalty))
-                    lb = seq.logit_bias or {}
-                    rb_lb_ids.extend(lb.keys())
-                    rb_lb_vals.extend(lb.values())
-                    rb_lb_off.append(len(rb_lb_ids))
-                    rb_out_toks.extend(seq.token_ids[seq.prompt_len:s0 + e.n])
-                    rb_out_off.append(len(rb_out_toks))
-            else:
-                bias_slot.append(-1)
-                freq_pen.append(0.0)
-                pres_pen.append(0.0)
-            if seq.repetition_penalty != 1.0:
-                need_penalty = True
-                if fresh:
-                    # everything known so far (prompt and the tokens generated before) becomes "seen"
-                    clear_slots.append(seq.slot)
-                    seen_rows.append(np.full(s0 + e.n, seq.slot, dtype=np.int32))
-                    seen_tokens.append(np.asarray(seq.token_ids[:s0 + e.n], dtype=np.int32))
-                else:
-                    seen_rows.append(np.full(e.n, seq.slot, dtype=np.int32))
-                    seen_tokens.append(np.asarray(seq.token_ids[s0:s0 + e.n], dtype=np.int32))
+                n = entries[i].n
+                seen_rows.append(np.full(n, seq.slot, dtype=np.int32))
+                seen_tokens.append(np.asarray(seq.token_ids[end - n:end], dtype=np.int32))
     mm = None
     if mrope:
         from gllm_b200.models.multimodal import batch_mm_payload
@@ -354,11 +367,12 @@ def build_batch(entries, page_size: int, vocab_size: int, batch_id: int = 0, mro
         logprobs_n=np.asarray(logprobs_n, dtype=np.int32) if want_logprobs else None,
         seed=np.asarray(seeds, dtype=np.int64) if want_seed else None,
         seed_pos=np.asarray(seed_pos, dtype=np.int32) if want_seed else None,
+        kv_copy=np.asarray(kv_copy, dtype=np.int32).reshape(-1, 2) if kv_copy else None,
         **(_bias_fields(freq_pen, pres_pen, bias_slot, rb_slots, rb_pen, rb_lb_off, rb_lb_ids, rb_lb_vals, rb_out_off,
                         rb_out_toks) if need_bias else {}),
         seq_ids=[e.seq.seq_id for e in entries] if n_dec == b else None,
         pt_gens=[e.seq.pt_gen for e in entries] if n_dec == b else None,
-        emit_ids=[entries[i].seq.seq_id for i in emit_seq])
+        emit_ids=emit_ids)
 
 
 class InputData:

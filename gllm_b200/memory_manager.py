@@ -51,13 +51,29 @@ class MemoryManager:
         # the LAST page is the dummy page (CUDA-graph padding rows read/write it)
         self.dummy_page: Optional[int] = self.id_allocator.allocate(num_pages - 1) if reserve_dummy_page else None
         self.usable_pages = num_pages - (1 if reserve_dummy_page else 0)
+        # page tables holding each page: several sequences share pages (prefix-cache hits, the prompt pages of the
+        # choices of a parallel-sampling request); a page returns to the free list when the last one lets go
+        self.page_ref: List[int] = [0] * num_pages
+        if self.dummy_page is not None:
+            self.page_ref[self.dummy_page] = 1
 
     # -- page accounting ------------------------------------------------------------------------
     def allocate_page(self) -> int:
-        return self.id_allocator.allocate()
+        page = self.id_allocator.allocate()
+        self.page_ref[page] += 1
+        return page
+
+    def share_page(self, page: int) -> int:
+        """One more page table holds `page` (already held by another one)."""
+        assert self.page_ref[page] > 0, page
+        self.page_ref[page] += 1
+        return page
 
     def free_page(self, page: int):
-        self.id_allocator.free(page)
+        assert self.page_ref[page] > 0, page
+        self.page_ref[page] -= 1
+        if self.page_ref[page] == 0:
+            self.id_allocator.free(page)
 
     def pages_needed(self, seq: Sequence) -> int:
         return max(0, (seq.seq_len + self.page_size - 1) // self.page_size - len(seq.page_table))
@@ -94,15 +110,12 @@ class MemoryManager:
 
 
 class PrefixMemoryManager(MemoryManager):
-    """Adds a hash -> page map with reference counts (automatic prefix caching)."""
+    """Adds a hash -> page map (automatic prefix caching); cached pages are shared through `page_ref`."""
 
     def __init__(self, num_pages: int, page_size: int, reserve_dummy_page: bool = False):
         super().__init__(num_pages, page_size, reserve_dummy_page)
         self.hash2page: Dict[int, int] = {}
         self.page2hash: List[Optional[int]] = [None] * num_pages
-        self.page_ref: List[int] = [0] * num_pages
-        if self.dummy_page is not None:
-            self.page_ref[self.dummy_page] = 1
         self.num_allocated_pages = 0
         self.num_hit_pages = 0
 
@@ -131,12 +144,6 @@ class PrefixMemoryManager(MemoryManager):
             self.hash2page[page_hash] = page
         self.page_ref[page] += 1
         return page
-
-    def free_page(self, page: int):
-        assert self.page_ref[page] > 0, page
-        self.page_ref[page] -= 1
-        if self.page_ref[page] == 0:
-            self.id_allocator.free(page)
 
     def pre_allocate_computed_page(self, seqs: List[Sequence]):
         """First touch of a sequence: reuse cached full pages of its prefix."""

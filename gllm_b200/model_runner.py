@@ -278,7 +278,9 @@ class ModelRunner:
         self.stats["steps"] += 1
         self.stats["tokens"] += batch.num_tokens
         bucket = None
-        if self.graphs and batch.is_decode_only() and batch.num_seqs <= self.capture_sizes[0]:
+        # (a fan-out batch has more sampled rows than sequences: the graphs produce one logits row per sequence)
+        if self.graphs and batch.is_decode_only() and batch.num_seqs <= self.capture_sizes[0] and \
+                batch.logits_idx.shape[0] == batch.num_seqs:
             bucket = min(b for b in self.graphs if b >= batch.num_seqs)
         inp.load(batch)
         if batch.feed_src is not None:
@@ -289,7 +291,10 @@ class ModelRunner:
             ev0 = torch.cuda.Event(enable_timing=True)
             ev0.record()
         try:
-            return self._step_loaded(batch, bucket, hidden, residual, recv_tiles)
+            res = self._step_loaded(batch, bucket, hidden, residual, recv_tiles)
+            if batch.kv_copy is not None:
+                self.copy_pages(batch.kv_copy)
+            return res
         finally:
             if self.time_steps and self.device.type == "cuda":
                 ev1 = torch.cuda.Event(enable_timing=True)
@@ -297,6 +302,18 @@ class ModelRunner:
                 kind = f"graph{bucket}" if bucket is not None else \
                     ("decode_eager" if batch.is_decode_only() else "prefill")
                 self._step_events.append((ev0, ev1, kind, batch.num_tokens))
+
+    def copy_pages(self, pairs):
+        """Parallel sampling: page dst := page src in every KV-cache tensor of this rank (its layers, its KV heads), in
+        stream order after the forward that wrote the src pages."""
+        kv = self.kv_cache
+        tensors = kv.k_cache + kv.v_cache
+        if self.device.type == "cuda":
+            from gllm_b200.ops import sm100 as ops
+        else:
+            from gllm_b200.ops import ref as ops
+        ops.kv_copy_pages(tensors, pairs.tolist(), dummy_page=self.num_pages - 1)
+        self.stats["kv_copy_pages"] = self.stats.get("kv_copy_pages", 0) + len(pairs)
 
     def gpu_busy_ms(self) -> float:
         """Sum of per-step device time (CUDA events around forward + sampling); resets the log."""

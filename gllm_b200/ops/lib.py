@@ -60,6 +60,7 @@ def _declare(lib):
     sig("gllm_silu_and_mul", [P, P, I, I, L, P])
     sig("gllm_embedding", [P, P, P, I, I, I, I, P])
     sig("gllm_gather_rows", [P, P, P, I, I, P])
+    sig("gllm_kv_copy_pages", [P, I, L, P, I, P])
     sig("gllm_rope_kv_write",
         [P, L, L, I, P, L, L, I, P, L, L, P, P, P, I, I, I, I, P, P, F, P, P, I, I, I, L, P])
     sig("gllm_attn_decode", [P, L, P, P, P, L, P, P, P, P, I, I, I, I, I, I, I, I, F, P, P])

@@ -23,6 +23,33 @@ def kv_cache_shape(num_pages: int, num_kv_heads: int, head_dim: int, page_size: 
     return (num_pages, num_kv_heads, head_dim // w, page_size, w)
 
 
+def check_copy_pairs(pairs, num_pages: int, dummy_page: Optional[int] = None):
+    """Validate (src, dst) page pairs of `kv_copy_pages` on the host: every page in [0, num_pages), the dst pages
+    distinct, no dst page also a src page (the copies of one launch run in any order), neither the dummy page."""
+    src = [int(s) for s, _ in pairs]
+    dst = [int(d) for _, d in pairs]
+    for p in src + dst:
+        if not 0 <= p < num_pages:
+            raise ValueError(f"kv_copy_pages: page {p} outside [0, {num_pages})")
+        if dummy_page is not None and p == dummy_page:
+            raise ValueError("kv_copy_pages: the dummy page is neither copied nor overwritten")
+    if len(set(dst)) != len(dst):
+        raise ValueError("kv_copy_pages: dst pages must be distinct")
+    if set(dst) & set(src):
+        raise ValueError("kv_copy_pages: a dst page is also a src page")
+
+
+def kv_copy_pages(tensors, pairs, dummy_page: Optional[int] = None):
+    """PyTorch model of csrc/elemwise/kv_copy.cu: for every page-major cache tensor, page dst := page src."""
+    if len(pairs) == 0:
+        return
+    check_copy_pairs(pairs, tensors[0].shape[0], dummy_page)
+    src = torch.tensor([int(s) for s, _ in pairs], dtype=torch.long)
+    dst = torch.tensor([int(d) for _, d in pairs], dtype=torch.long)
+    for t in tensors:
+        t[dst.to(t.device)] = t[src.to(t.device)]
+
+
 # ----------------------------------------------------------------------------------------------
 # dense ops
 # ----------------------------------------------------------------------------------------------

@@ -491,6 +491,40 @@ def bias_rebuild(bias: torch.Tensor, out_seen: torch.Tensor, v: int, slots: torc
     _count()
 
 
+_kv_bases = {}
+
+
+def kv_copy_pages(tensors, pairs, dummy_page: Optional[int] = None):
+    """For every page-major KV-cache tensor of this rank (K and V of each layer, or the MLA latent): page dst := page
+    src for each (src, dst) in `pairs`, in one launch (csrc/elemwise/kv_copy.cu). The pairs are checked on the host
+    first (`ref.check_copy_pairs`). The device array of layer base pointers is built once per set of tensors."""
+    if len(pairs) == 0:
+        return
+    from gllm_b200.ops.ref import check_copy_pairs
+    t0 = tensors[0]
+    check_copy_pairs(pairs, t0.shape[0], dummy_page)
+    for t in tensors:
+        assert t.is_cuda and t.is_contiguous() and t.shape == t0.shape and t.dtype == t0.dtype
+        assert t.data_ptr() % 16 == 0
+    key = tuple(t.data_ptr() for t in tensors)
+    bases = _kv_bases.get(key)
+    if bases is None:
+        bases = torch.tensor(list(key), dtype=torch.int64).to(t0.device)
+        _kv_bases[key] = bases
+    # (pinned staging: a copy from pageable memory would make the host wait for the work queued before it)
+    host = torch.tensor([[int(s), int(d)] for s, d in pairs], dtype=torch.int32).pin_memory()
+    launch_kv_copy_pages(tensors, bases, host.to(t0.device, non_blocking=True))
+
+
+def launch_kv_copy_pages(tensors, bases: torch.Tensor, dev_pairs: torch.Tensor):
+    """The launch alone: `bases` int64 [len(tensors)] and `dev_pairs` int32 [n, 2] already on the device and checked."""
+    t0 = tensors[0]
+    L = _lib.load()
+    check(L.gllm_kv_copy_pages(_p(bases), len(tensors), t0[0].numel() * t0.element_size(), _p(dev_pairs),
+                               dev_pairs.shape[0], stream_ptr()), "kv_copy_pages")
+    _count()
+
+
 def mark_seen(seen_bits: torch.Tensor, rows: torch.Tensor, tokens: torch.Tensor):
     assert rows.dtype == torch.int32 and tokens.dtype == torch.int32
     L = _lib.load()

@@ -64,7 +64,7 @@ PLACEHOLDER = -1  # token id of a position whose value is still being sampled on
 
 class ScheduledSeq:
     """One entry of a micro-batch: compute tokens [start, start + n) of `seq`."""
-    __slots__ = ("seq", "start", "n", "emits", "is_decode")
+    __slots__ = ("seq", "start", "n", "emits", "is_decode", "forks", "kv_copy")
 
     def __init__(self, seq: Sequence, start: int, n: int):
         self.seq, self.start, self.n = seq, start, n
@@ -73,6 +73,11 @@ class ScheduledSeq:
         # `computed_token_num >= prompt_len` test would emit early on a chunked recompute.)
         self.emits = start + n >= len(seq.token_ids)
         self.is_decode = n == 1 and self.emits and start >= seq.prompt_len
+        # parallel sampling: the other choices whose first tokens are drawn from this entry's last logits row (one
+        # extra sampled row each, after every entry's own row) and the (src, dst) page copies that give each of them
+        # the partial last prompt page. None for every other entry.
+        self.forks: Optional[List[Sequence]] = None
+        self.kv_copy: Optional[List[tuple]] = None
 
     def __repr__(self):
         return f"ScheduledSeq(id={self.seq.seq_id}, start={self.start}, n={self.n})"
@@ -137,6 +142,8 @@ class Scheduler:
                 logger.warning("request %d: output capped to %d tokens (KV cache holds %d tokens)", seq.seq_id,
                                cap - len(seq), cap)
                 seq.output_len = cap - len(seq)
+            for sib in seq.forks:
+                sib.output_len = min(sib.output_len, max(cap - len(seq), 1))
         self.seqs_to_prefill.extend(seqs)
 
     def add_abort_ids(self, ids):
@@ -172,6 +179,8 @@ class Scheduler:
         if next_logprobs is not None:
             out.next_logprobs = []
         prefix, ps = isinstance(self.mm, PrefixMemoryManager), self.page_size
+        if any(ent.forks for ent in batch):
+            self._process_forks(batch, next_tokens, next_logprobs, out)
         k = 0  # next_tokens holds one token per *emitting* entry, in batch order
         for ent in batch:
             seq = ent.seq
@@ -228,6 +237,61 @@ class Scheduler:
                     self.seqs_to_decode.appendleft(seq)
             # else: unfinished prefill — its continuation is already at the head of seqs_to_prefill
         return out
+
+    def _process_forks(self, batch, next_tokens, next_logprobs, out: SchedulerOutput):
+        """The extra rows of a fan-out follow every entry's own row: hand token i to choice i. Runs before the
+        entries' own tokens, so it is done before the parent can be freed (it may finish on its first token)."""
+        k = sum(1 for ent in batch if ent.emits)
+        for ent in batch:
+            for sib in ent.forks or ():
+                tok = int(next_tokens[k])
+                lp = next_logprobs[k] if next_logprobs is not None else None
+                k += 1
+                if sib.is_abort or sib.seq_id in self.abort_ids:
+                    sib.is_abort = True
+                    self.mm.free(sib)
+                    out.free_ids.append(sib.seq_id)
+                    self.abort_ids.discard(sib.seq_id)
+                    continue
+                sib.append(tok)
+                out.act_schedule_ids.append(sib.seq_id)
+                out.next_tokens.append(tok)
+                if next_logprobs is not None:
+                    out.next_logprobs.append(lp)
+                if (not sib.ignore_eos and tok in sib.finish_tokens) or \
+                        len(sib.token_ids) - sib.prompt_len >= sib.output_len:
+                    out.free_ids.append(sib.seq_id)
+                    self.mm.free(sib)
+                else:
+                    self.seqs_to_decode.appendleft(sib)
+
+    def _fan_out(self, ent: "ScheduledSeq"):
+        """The final prompt chunk of a sequence with forks is scheduled (its pages are allocated): every fork takes
+        the F full prompt pages (shared, reference counted: nobody writes them again) and, when the prompt ends
+        inside a page, a fresh page that the device fills with a copy of page F right after this batch's forward."""
+        seq, ps = ent.seq, self.page_size
+        p = len(seq.token_ids)
+        full = p // ps
+        pairs = []
+        for sib in seq.forks:
+            sib.page_table = [self.mm.share_page(pg) for pg in seq.page_table[:full]]
+            if p % ps:
+                dst = self.mm.allocate_page()
+                sib.page_table.append(dst)
+                pairs.append((seq.page_table[full], dst))
+            sib.computed_token_num = sib.scheduled_token_num = p
+            sib.published = full     # the shared pages are the parent's to publish
+        ent.forks, ent.kv_copy = seq.forks, (pairs or None)
+        seq.forks = []
+
+    def _abort_forks(self, seq: Sequence, everything: bool, out: SchedulerOutput):
+        """Forks still waiting with their parent (before its fan-out): drop the aborted ones, or all of them."""
+        for sib in list(seq.forks):
+            if everything or sib.seq_id in self.abort_ids:
+                seq.forks.remove(sib)
+                sib.is_abort = True
+                out.free_ids.append(sib.seq_id)
+                self.abort_ids.discard(sib.seq_id)
 
     def _in_flight(self, seq: Sequence) -> bool:
         return any(e.seq is seq for b in self.batch_running for e in b)
@@ -306,6 +370,8 @@ class Scheduler:
         inflight = {id(e.seq) for b in self.batch_running for e in b}
         for q in (self.seqs_to_prefill, self.seqs_to_decode):
             for seq in list(q):
+                if seq.forks:
+                    self._abort_forks(seq, seq.seq_id in self.abort_ids, out)
                 if seq.seq_id in self.abort_ids:
                     q.remove(seq)
                     seq.is_abort = True
@@ -320,6 +386,9 @@ class Scheduler:
                 if ent.seq.seq_id in self.abort_ids:
                     ent.seq.is_abort = True
                     live.add(ent.seq.seq_id)
+                for sib in ent.forks or ():      # fanned out in flight: freed when that batch returns
+                    if sib.seq_id in self.abort_ids:
+                        live.add(sib.seq_id)
         # an abort that matches nothing alive (the sequence finished just before, or was never admitted) must not
         # linger: it would disable lookahead scheduling for good and hit a later request that re-uses the id
         self.abort_ids &= live
@@ -401,7 +470,8 @@ class Scheduler:
         """`room`: how many more sequences the micro-batch may take (None = unlimited)."""
         batch: List[ScheduledSeq] = []
         n_tokens = 0
-        while self.seqs_to_prefill and budget > 0 and (room is None or len(batch) < room):
+        fork_rows = 0    # extra sampled rows of the fan-outs in this batch (each takes a sequence slot of the runner)
+        while self.seqs_to_prefill and budget > 0 and (room is None or len(batch) + fork_rows < room):
             seq = self.seqs_to_prefill[0]
             if isinstance(self.mm, PrefixMemoryManager) and seq.scheduled_token_num == 0 and not seq.page_table:
                 self.mm.pre_allocate_computed_page([seq])
@@ -409,13 +479,24 @@ class Scheduler:
             remaining = len(seq) - start
             take = min(remaining, budget)
             seq.scheduled_token_num = start + take
-            if self.mm.pages_needed(seq) > self.mm.get_num_free_pages():
+            fan = seq.forks if take == remaining else None
+            need = self.mm.pages_needed(seq)
+            if fan:
+                need += len(fan) if len(seq) % self.page_size else 0
+                if room is not None and len(batch) + fork_rows + 1 + len(fan) > room:
+                    seq.scheduled_token_num = start
+                    break  # no room for the choices' rows in this batch: the chunk waits
+            if need > self.mm.get_num_free_pages():
                 seq.scheduled_token_num = start
                 break  # no KV room right now
             self.mm.pre_allocate_page([seq])
             n_tokens += take
             budget -= take
-            batch.append(ScheduledSeq(seq, start, take))
+            ent = ScheduledSeq(seq, start, take)
+            if fan:
+                self._fan_out(ent)
+                fork_rows += len(ent.forks)
+            batch.append(ent)
             if take == remaining:
                 self.seqs_to_prefill.popleft()
             # else: unfinished prefill stays at the queue head and continues with its next chunk —

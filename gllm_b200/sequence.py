@@ -11,7 +11,7 @@ class Sequence:
                  "mm_contents", "page_hashes", "num_cached_tokens", "arrival_time", "first_token_time",
                  "finish_time", "slot", "mrope_delta", "mm_state", "pt_np", "pending", "zombie", "pt_gen", "published",
                  "slot_fresh", "logprobs", "output_logprobs", "seed", "frequency_penalty", "presence_penalty",
-                 "logit_bias")
+                 "logit_bias", "forks")
 
     def __init__(self, seq_id: int, token_ids: List[int], finish_tokens: List[int],
                  output_len: Optional[int] = None, ignore_eos: bool = False, temperature: float = 0.6,
@@ -65,6 +65,10 @@ class Sequence:
         self.pending = -1    # index of a placeholder token reserved by a lookahead step (async scheduling)
         self.zombie = False  # finished while a lookahead step was already in flight: pages freed when it returns
         self.mm_state = None
+        # parallel sampling (`n` > 1): the other choices of this request. They travel with this sequence (choice 0)
+        # and are not scheduled on their own: when its final prompt chunk is scheduled they take its full prompt
+        # pages, a copy of its partial last page, and first tokens drawn from its last logits row. Emptied then.
+        self.forks: List["Sequence"] = []
 
     @property
     def has_bias_row(self) -> bool:
