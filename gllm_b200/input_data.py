@@ -89,6 +89,11 @@ class BatchArrays:
     def is_decode_only(self) -> bool:
         return self.num_decode_seqs == self.num_seqs
 
+    @property
+    def plain_greedy(self) -> bool:
+        """Every emitting row takes the argmax of its raw logits: no penalty, bias or sampling parameter to apply."""
+        return self.all_greedy and not self.need_penalty and not self.need_bias
+
     def to_wire(self):
         """(header dict, [one contiguous buffer]) for zero-copy IPC: every array is packed into a single blob
         (16-byte aligned sections) so a batch costs two zmq frames per peer instead of one per array."""
@@ -466,7 +471,7 @@ class InputData:
         if self.num_emit:
             self._put(self._logits_idx, batch.logits_idx)
             # the greedy argmax path of the sm_90a sampler reads none of these
-            if not (self.device.type == "cuda" and batch.all_greedy and not batch.need_penalty and not batch.need_bias):
+            if not (self.device.type == "cuda" and batch.plain_greedy):
                 self._put(self._temperature, batch.temperature)
                 self._put(self._top_k, batch.top_k)
                 self._put(self._top_p, batch.top_p)

@@ -5,10 +5,6 @@ PyTorch oracle (`ops.ref`) — that is the CPU plumbing/test path only, never a 
 """
 from __future__ import annotations
 
-from typing import Optional
-
-import torch
-
 from gllm_b200.ops import ref
 
 
@@ -84,32 +80,3 @@ def paged_attention(q, k_cache, v_cache, inp, scale, num_q_heads, head_dim):
     return ref.paged_attention(q, k_cache, v_cache, inp.block_table, inp.seq_lens, inp.query_start_loc, scale,
                                num_q_heads, head_dim)
 
-
-def sample(logits, inp, seen_bits=None, seed=0, step=None, bias_rows=None):
-    """`bias_rows`: the runner's per-slot frequency / presence / logit_bias rows when some row of the batch has one
-    (`inp.bias_slot`); seeded rows (`inp.seeds`) draw from their own (seed, position) stream."""
-    b = logits.shape[0]
-    bslot = inp.bias_slot if bias_rows is not None else None
-    seeds, spos = inp.seeds
-    if logits.is_cuda:
-        sm = _sm()
-        if inp.batch is not None and inp.batch.all_greedy and not inp.batch.need_penalty and bslot is None:
-            return sm.sample(logits)
-        return sm.sample(logits, inp.temperature[:b], inp.top_k[:b], inp.top_p[:b],
-                         inp.rep_penalty[:b] if seen_bits is not None else None, seen_bits,
-                         inp.state_slot[:b] if seen_bits is not None else None, seed=seed, step=step,
-                         bias=bias_rows if bslot is not None else None, bias_slot=bslot, seeds=seeds, seed_pos=spos)
-    seen_mask = None
-    if seen_bits is not None:
-        v = logits.shape[1]
-        rows = seen_bits[inp.state_slot[:b].long()]
-        bits = (rows.unsqueeze(-1) >> torch.arange(32, dtype=torch.int32)) & 1
-        seen_mask = bits.reshape(b, -1)[:, :v].bool()
-    bias = None
-    if bslot is not None:
-        bias = bias_rows[bslot.clamp(min=0).long(), : logits.shape[1]].clone()
-        bias[bslot < 0] = 0.0
-    g = torch.Generator().manual_seed(seed + (int(step) if step is not None else 0))
-    return ref.sample(logits, inp.temperature[:b], inp.top_k[:b], inp.top_p[:b],
-                      inp.rep_penalty[:b] if seen_bits is not None else None, seen_mask, generator=g, bias=bias,
-                      seeds=seeds, seed_pos=spos)

@@ -1,7 +1,7 @@
 """Worker-side model execution (reference: gllm/model_runner.py:165-478).
 
 Owns: this rank's model slice, the paged KV cache, the persistent `InputData`, static PP
-activation buffers, CUDA graphs for decode-only batches, and the sampler state.
+activation buffers, CUDA graphs for decode-only batches, and the `Sampler`.
 
     runner.init()                                  load / profile / size KV / capture graphs
     runner.step(batch, hidden=None, residual=None) one micro-batch through this stage
@@ -21,11 +21,11 @@ import torch
 
 from gllm_b200.config import EngineConfig, capture_sizes
 from gllm_b200.input_data import BatchArrays, InputData
-from gllm_b200.layers import functional as Fn
 from gllm_b200.memory_manager import KVCache
 from gllm_b200.model_loader import ModelLoader
 from gllm_b200.parallel import state as ps
 from gllm_b200.parallel.tp import make_tp_comm
+from gllm_b200.sampler import Sampler
 from gllm_b200.utils.logging import logger
 
 
@@ -90,10 +90,7 @@ class ModelRunner:
         self.graphs: Dict[int, object] = {}
         self.num_pages = 0
         self.device = None
-        self.seen_bits = None
-        self.bias_rows = None    # fp32 [slots, V]: frequency / presence penalties + logit_bias (`_bias_state`)
-        self.out_seen = None     # int32 [slots, ceil(V/32)]: tokens each slot's sequence has generated
-        self.step_counter = None
+        self.sampler: Optional[Sampler] = None
         self.stats = {"steps": 0, "graph_steps": 0, "tokens": 0, "h2d_bytes": 0, "d2h_bytes": 0,
                       "graph_kernel_launches": 0, "gpu_ms": 0.0}
         self.graph_kernels: Dict[int, int] = {}
@@ -133,13 +130,12 @@ class ModelRunner:
         self.input_data = InputData(self.max_num_batched_tokens, max(self.max_running_seqs, 1), max_blocks,
                                     self.device, mrope=mrope)
         self.input_data.need_tok_seq = bool(self.loader.use_mla)
-        # vocab-parallel sampling: the forward (and its CUDA graphs) ends at this rank's logits shard
         # test hook (tests/mp_tp_check.py): keep the full last-token logits of every step, per emitting sequence id
         self.keep_logits = os.environ.get("GLLM_KEEP_LOGITS", "0") == "1"
         self.logit_log = []
-        self.vp_sample = cfg.tp_size > 1 and os.environ.get("GLLM_VP_SAMPLE", "1") != "0"
-        # GLLM_VP_SAMPLE=greedy: vocab-parallel argmax only, sampled batches all-gather the logits (the round-1 path)
-        self.vp_candidates = os.environ.get("GLLM_VP_SAMPLE", "1") != "greedy"
+        # vocab-parallel sampling: the forward (and its CUDA graphs) ends at this rank's logits shard
+        self.sampler = Sampler(self.device, self.spec.vocab_size, cfg.seed, self.input_data, self.stats,
+                               vocab_parallel=cfg.tp_size > 1 and os.environ.get("GLLM_VP_SAMPLE", "1") != "0")
         h, dt = self.spec.hidden_size, self.spec.dtype
         if not ps.is_first_pp_rank():
             self.input_hidden = torch.zeros(self.max_num_batched_tokens, h, dtype=dt, device=self.device)
@@ -154,7 +150,6 @@ class ModelRunner:
             self._host_flip = 0
             self.tokens_host = self._tokens_host2[0]
             self._lp_host2 = None        # pinned log-prob result buffers, allocated on the first request that asks
-            self.step_counter = torch.zeros(1, dtype=torch.int64, device=self.device)
         logger.info("model loaded in %.1fs", time.time() - t0)
         self.profile_run()
         self.num_pages = self.compute_num_pages()
@@ -221,7 +216,8 @@ class ModelRunner:
         else:
             h, r = self.model(inp, kv, self.tpc, hidden, residual)
         if ps.is_last_pp_rank():
-            return self.model.compute_logits(inp, h, self.tpc, all_rows=all_rows, local=self.vp_sample), None
+            vp = self.sampler.vocab_parallel
+            return self.model.compute_logits(inp, h, self.tpc, all_rows=all_rows, local=vp), None
         return h, r
 
     def capture_graphs(self):
@@ -307,12 +303,7 @@ class ModelRunner:
         """Parallel sampling: page dst := page src in every KV-cache tensor of this rank (its layers, its KV heads), in
         stream order after the forward that wrote the src pages."""
         kv = self.kv_cache
-        tensors = kv.k_cache + kv.v_cache
-        if self.device.type == "cuda":
-            from gllm_b200.ops import sm100 as ops
-        else:
-            from gllm_b200.ops import ref as ops
-        ops.kv_copy_pages(tensors, pairs.tolist(), dummy_page=self.num_pages - 1)
+        self.sampler.ops.kv_copy_pages(kv.k_cache + kv.v_cache, pairs.tolist(), dummy_page=self.num_pages - 1)
         self.stats["kv_copy_pages"] = self.stats.get("kv_copy_pages", 0) + len(pairs)
 
     def gpu_busy_ms(self) -> float:
@@ -356,218 +347,14 @@ class ModelRunner:
         return StepResult(hidden=out, residual=r)
 
     def _sample(self, batch: BatchArrays, logits: torch.Tensor) -> StepResult:
-        inp = self.input_data
         e = logits.shape[0]
         if e == 0:
             return StepResult(tokens=self.tokens_out[:0], num_emit=0)
         if self.keep_logits:
-            full = self.tpc.gather_logits(logits, self.spec.vocab_size) if self.vp_sample else logits
+            full = self.tpc.gather_logits(logits, self.spec.vocab_size) if self.sampler.vocab_parallel else logits
             self.logit_log.append((list(batch.emit_ids or []), full[:e, : self.spec.vocab_size].float().cpu()))
-        bias = None
-        if batch.need_bias:
-            bias = self._bias_state(int(batch.bias_slot.max()) + 1)
-            if batch.rb_slots is not None:
-                self._rebuild_bias(batch)
-        if self.vp_sample and batch.all_greedy and not batch.need_penalty and not batch.need_bias:
-            toks = self._vp_greedy(logits)
-            return self._finish_sample(toks, e, self._logprobs(batch, logits, toks, vocab_parallel=True))
-        if self.vp_sample and not self.vp_candidates:
-            logits = self.tpc.gather_logits(logits, self.spec.vocab_size)   # GLLM_VP_SAMPLE=greedy: A/B switch
-        seen = None
-        if batch.need_penalty:
-            seen = self._seen_bits(int(batch.state_slot.max()) + 1 if len(batch.state_slot) else 1)
-            dev = self.device
-            if batch.clear_slots is not None:
-                seen[torch.from_numpy(batch.clear_slots).to(dev).long()] = 0
-            if batch.seen_rows is not None:
-                rows = torch.from_numpy(batch.seen_rows).to(dev)
-                toks = torch.from_numpy(batch.seen_tokens).to(dev)
-                if dev.type == "cuda":
-                    from gllm_b200.ops import sm100
-                    sm100.mark_seen(seen, rows, toks)
-                else:
-                    word = (toks >> 5).long()
-                    bit = (torch.ones_like(toks) << (toks & 31)).to(torch.int32)
-                    for rw, wd, bt in zip(rows.tolist(), word.tolist(), bit.tolist()):
-                        seen[rw, wd] |= bt
-        if not batch.all_greedy:
-            self.step_counter += 1
-        if self.vp_sample and self.vp_candidates:
-            toks = self._vp_sample(logits, seen, bias)
-            self._account_bias(batch, toks)
-            return self._finish_sample(toks, e, self._logprobs(batch, logits, toks, vocab_parallel=True))
-        toks = Fn.sample(logits, inp, seen, seed=self.cfg.seed, step=self.step_counter, bias_rows=bias)
-        self._account_bias(batch, toks)
-        return self._finish_sample(toks, e, self._logprobs(batch, logits, toks, vocab_parallel=False))
-
-    def _bias_state(self, rows: int) -> torch.Tensor:
-        """[rows, V] fp32 bias rows (and the [rows, V/32] output-token bitmask), one per slot; grown (never shrunk)
-        like `_seen_bits`. About V * 4.125 bytes per slot (594 KiB at V = 151936); not part of the KV-cache sizing."""
-        if self.bias_rows is None or self.bias_rows.shape[0] < rows:
-            v = self.spec.vocab_size
-            n = max(rows, 65 if self.bias_rows is None else 2 * self.bias_rows.shape[0])
-            b = torch.zeros(n, v, dtype=torch.float32, device=self.device)
-            o = torch.zeros(n, (v + 31) // 32, dtype=torch.int32, device=self.device)
-            if self.bias_rows is not None:
-                b[: self.bias_rows.shape[0]] = self.bias_rows
-                o[: self.out_seen.shape[0]] = self.out_seen
-            self.bias_rows, self.out_seen = b, o
-        return self.bias_rows
-
-    def _rebuild_bias(self, batch: BatchArrays):
-        """Slots (re)assigned this step: clear, scatter logit_bias, replay the counts of the outputs known so far."""
-        dev = self.device
-        if dev.type == "cuda":
-            from gllm_b200.ops import sm100
-            t = [torch.from_numpy(np.ascontiguousarray(a)).to(dev) for a in
-                 (batch.rb_slots, batch.rb_pen, batch.rb_lb_off, batch.rb_lb_ids, batch.rb_lb_vals, batch.rb_out_off,
-                  batch.rb_out_toks)]
-            sm100.bias_rebuild(self.bias_rows, self.out_seen, self.spec.vocab_size, *t)
-            return
-        from gllm_b200.ops import ref
-        lo, oo = batch.rb_lb_off, batch.rb_out_off
-        for r, slot in enumerate(batch.rb_slots.tolist()):
-            ref.bias_rebuild(self.bias_rows, self.out_seen, slot, float(batch.rb_pen[r, 0]), float(batch.rb_pen[r, 1]),
-                             batch.rb_lb_ids[lo[r]:lo[r + 1]], batch.rb_lb_vals[lo[r]:lo[r + 1]],
-                             batch.rb_out_toks[oo[r]:oo[r + 1]].tolist())
-
-    def _account_bias(self, batch: BatchArrays, toks: torch.Tensor):
-        """After the tokens are chosen: every emitting row with a bias row charges its token, on the device — the host
-        never sends per-step tokens, so these rows stay eligible for lookahead and the incremental decode path."""
-        if not batch.need_bias:
-            return
-        inp = self.input_data
-        if toks.is_cuda:
-            from gllm_b200.ops import sm100
-            sm100.bias_account(self.bias_rows, self.out_seen, inp.bias_slot, toks.to(torch.int32).contiguous(),
-                               inp.freq_pen, inp.pres_pen)
-            return
-        from gllm_b200.ops import ref
-        for r, (slot, tok) in enumerate(zip(inp.bias_slot.tolist(), toks.tolist())):
-            if slot >= 0:
-                ref.bias_account_one(self.bias_rows, self.out_seen, slot, int(tok), float(inp.freq_pen[r]),
-                                     float(inp.pres_pen[r]))
-
-    def _logprobs(self, batch: BatchArrays, logits: torch.Tensor, toks: torch.Tensor,
-                  vocab_parallel: bool) -> Optional[torch.Tensor]:
-        """Log-probabilities of the raw model distribution for the emitting rows that asked (csrc/sample/sampler.cu:
-        logprobs_shard_kernel / logprobs_final_kernel), after the tokens are chosen. `vocab_parallel`: `logits` is this
-        rank's vocab shard — every TP rank reduces its shard to [E_lp, 2N+3] records and the ranks all-gather them
-        (every rank decides from the batch alone, so all of them join the collective). None when no row asked: then
-        the step launches, exchanges and copies nothing more than without this feature."""
-        lpn = batch.logprobs_n
-        if lpn is None:
-            return None
-        want = np.nonzero(lpn >= 0)[0].astype(np.int32)
-        if want.size == 0:
-            return None
-        n = int(lpn[want].max())
-        rows = torch.from_numpy(want).to(logits.device)
-        toks = toks.to(torch.int32).contiguous()
-        v_full = self.spec.vocab_size
-        tp, off, valid = 1, 0, v_full
-        if vocab_parallel:
-            st = ps.get_state()
-            per = logits.shape[1]
-            tp, off = st.tp_size, st.tp_rank * per
-            valid = max(0, min(per, v_full - off))   # the last rank's shard ends with padding columns
-        if logits.is_cuda:
-            from gllm_b200.ops import sm100 as ops
-        else:
-            from gllm_b200.ops import ref as ops
-        rec = ops.logprobs_shard(logits, valid, n, toks, rows, vocab_offset=off)
-        if tp > 1:
-            import torch.distributed as dist
-            allr = torch.empty(tp, *rec.shape, dtype=torch.float32, device=rec.device)
-            dist.all_gather_into_tensor(allr.view(tp * rec.shape[0], rec.shape[1]), rec, group=ps.get_state().tp_group)
-        else:
-            allr = rec.unsqueeze(0)
-        self.stats["logprob_rows"] = self.stats.get("logprob_rows", 0) + len(want)
-        return ops.logprobs_final(allr, n)
-
-    VP_CANDIDATES = 256   # per rank and row; top_k <= this is exact (csrc/sample/sampler.cu)
-
-    def _vp_sample(self, shard: torch.Tensor, seen: Optional[torch.Tensor],
-                   bias: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """Vocab-parallel top-k / top-p / penalty sampling (SURVEY §2.4 X4): every rank reduces its vocab shard to
-        a [E, 2C+4] record (C best candidates, softmax statistics, race winner), the ranks all-gather the records —
-        ~2 KB per row and rank instead of V/tp logits — and finish on the tp x C candidates with the exact global
-        normalisation. The [E, V] logits are never materialised (the reference all-gathers them and sorts the full
-        vocabulary: gllm/layers/vocab_parallel_embedding.py:423-435, gllm/layers/sampler.py:8-54)."""
-        import torch.distributed as dist
-        inp = self.input_data
-        e, per = shard.shape
-        st = ps.get_state()
-        r0 = st.tp_rank * per
-        v_full = self.spec.vocab_size
-        valid = max(0, min(per, v_full - r0))
-        c = min(self.VP_CANDIDATES, per)
-        pen = inp.rep_penalty[:e] if seen is not None else None
-        seeds, spos = inp.seeds
-        bslot = inp.bias_slot if bias is not None else None
-        if shard.is_cuda:
-            from gllm_b200.ops import sm100
-            rec = sm100.vp_candidates(shard, valid, v_full, c, inp.temperature[:e], inp.top_k[:e], inp.top_p[:e],
-                                      pen, seen, inp.state_slot[:e] if seen is not None else None,
-                                      seed=self.cfg.seed, step=self.step_counter, vocab_offset=r0,
-                                      bias=bias if bslot is not None else None, bias_slot=bslot, seeds=seeds,
-                                      seed_pos=spos)
-        else:
-            from gllm_b200.ops import ref
-            step = int(self.step_counter) if self.step_counter is not None else 0
-            g = torch.Generator().manual_seed(self.cfg.seed + step)
-            race = torch.empty(e, per * st.tp_size).exponential_(1.0, generator=g)[:, r0:r0 + max(valid, 0)]
-            if seeds is not None:       # seeded rows: the kernel's stream, keyed by token id
-                for r in np.nonzero(spos.numpy() >= 0)[0].tolist():
-                    race[r] = ref.race_exp(int(seeds[r]), int(spos[r]), range(r0, r0 + max(valid, 0)))
-            dense = _dense_bias(bias, bslot, r0 + max(valid, 0))
-            dense = dense[:, r0:] if dense is not None else None
-            mask = None
-            if seen is not None:
-                rows = seen[inp.state_slot[:e].long()]
-                bits = (rows.unsqueeze(-1) >> torch.arange(32, dtype=torch.int32)) & 1
-                full = bits.reshape(e, -1).bool()
-                if full.shape[1] < r0 + valid:
-                    full = torch.nn.functional.pad(full, (0, r0 + valid - full.shape[1]))
-                mask = full[:, r0:r0 + valid]
-            rec = ref.vp_candidates(shard, valid, v_full, c, inp.temperature[:e], inp.top_k[:e], inp.top_p[:e], pen,
-                                    mask, race, vocab_offset=r0, bias=dense)
-        allr = torch.empty(st.tp_size, e, 2 * c + 4, dtype=torch.float32, device=shard.device)
-        dist.all_gather_into_tensor(allr.view(st.tp_size * e, 2 * c + 4), rec, group=st.tp_group)
-        self.stats["vp_sample_steps"] = self.stats.get("vp_sample_steps", 0) + 1
-        if shard.is_cuda:
-            return sm100.vp_final(allr, c, v_full, inp.top_k[:e], inp.top_p[:e], seed=self.cfg.seed,
-                                  step=self.step_counter, seeds=seeds, seed_pos=spos)
-        g = torch.Generator().manual_seed(self.cfg.seed + step + 0x5bd1)
-        return ref.vp_final(allr, c, v_full, inp.top_k[:e], inp.top_p[:e], generator=g, seeds=seeds, seed_pos=spos)
-
-    def _vp_greedy(self, shard: torch.Tensor) -> torch.Tensor:
-        """Vocab-parallel greedy sampling (SURVEY §2.4 X4): every rank takes the argmax of its own vocab shard
-        with the sampler kernel, the ranks exchange (value, global index) pairs — 8 bytes per row instead of the
-        [E, V] logits — and pick the winner (lowest rank on ties == lowest token id)."""
-        import torch.distributed as dist
-        e, per = shard.shape
-        st = ps.get_state()
-        r0 = st.tp_rank * per
-        valid = max(0, min(per, self.spec.vocab_size - r0))   # the last rank's shard ends with padding rows
-        pack = torch.empty(e, 2, dtype=torch.float32, device=shard.device)
-        if valid > 0:
-            if shard.is_cuda:
-                from gllm_b200.ops import sm100
-                val = torch.empty(e, dtype=torch.float32, device=shard.device)
-                idx = sm100.sample(shard[:, :valid], out_max=val, vocab_offset=r0)
-            else:
-                val, idx = shard[:, :valid].float().max(dim=1)
-                idx = idx + r0
-            pack[:, 0] = val
-            pack[:, 1] = idx.float()   # token ids < 2^24 are exact in fp32
-        else:
-            pack[:, 0] = float("-inf")
-            pack[:, 1] = 0
-        allp = torch.empty(st.tp_size, e, 2, dtype=torch.float32, device=shard.device)
-        dist.all_gather_into_tensor(allp.view(st.tp_size * e, 2), pack, group=st.tp_group)
-        best = allp[:, :, 0].argmax(dim=0, keepdim=True)
-        return allp[:, :, 1].gather(0, best)[0].to(torch.int32)
+        toks, logprobs = self.sampler.sample(batch, logits)
+        return self._finish_sample(toks, e, logprobs)
 
     def _finish_sample(self, toks: torch.Tensor, e: int, logprobs: Optional[torch.Tensor] = None) -> StepResult:
         self.tokens_out[:e].copy_(toks)
@@ -605,27 +392,6 @@ class ModelRunner:
         tpc, self.tpc = self.tpc, None
         if tpc is not None and hasattr(tpc, "close"):
             tpc.close()
-
-    def _seen_bits(self, rows: int = 1):
-        """[rows, V/32] seen-token bitmask, one row per sequence holding penalty state (row 0: none). Grown (never
-        shrunk) to cover the largest row the driver has handed out: every rank sees the same `state_slot`."""
-        if self.seen_bits is None or self.seen_bits.shape[0] < rows:
-            words = (self.spec.vocab_size + 31) // 32
-            n = max(rows, 65 if self.seen_bits is None else 2 * self.seen_bits.shape[0])
-            new = torch.zeros(n, words, dtype=torch.int32, device=self.device)
-            if self.seen_bits is not None:
-                new[: self.seen_bits.shape[0]] = self.seen_bits
-            self.seen_bits = new
-        return self.seen_bits
-
-
-def _dense_bias(bias_rows: Optional[torch.Tensor], bias_slot: Optional[torch.Tensor], v: int):
-    """CPU path: [E, v] additive rows of the emitting rows (zeros where a row has none), or None."""
-    if bias_rows is None or bias_slot is None:
-        return None
-    rows = bias_rows[bias_slot.clamp(min=0).long(), :v].clone()
-    rows[bias_slot < 0] = 0.0
-    return rows
 
 
 def _dummy_batch(num_tokens: int, num_seqs: int, page_size: int, max_blocks: int, page: int = 0,
