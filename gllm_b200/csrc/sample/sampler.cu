@@ -657,6 +657,104 @@ logprobs_final_kernel(const float* __restrict__ gathered, int tp, int E, int N, 
   }
 }
 
+// ------------------------------------------------------------------------------------------------------------------
+// Prompt log-probabilities (scoring): Q rows of LM-head logits, each with its own target token (the next prompt
+// token). Q is a whole prompt, far more rows than the sampled ones, and a tile of them does not stay in L2 for
+// the 2 - 7 passes of logprobs_shard_kernel. For N <= 1 (perplexity, and the is-greedy check of evaluation
+// harnesses) one pass over the row suffices: an online max / sum-exp with rescaling, a running argmax (ties to the
+// lower token id, as block_argmax) and the target's raw logit. The record is logprobs_shard_kernel's [2N+3] layout,
+// so the all-gather and logprobs_final_kernel are shared. Rows with N > 1 take logprobs_shard_kernel.
+// ------------------------------------------------------------------------------------------------------------------
+static constexpr int kPromptLpThreads = 512;
+
+// (m, s) of a set of logits: s = sum exp(x - m). Merging with m = -inf (an empty or all -inf set) adds nothing.
+__device__ __forceinline__ void lse_merge(float& m, float& s, float m2, float s2) {
+  if (m2 == -INFINITY) return;
+  if (m == -INFINITY) { m = m2; s = s2; return; }
+  if (m2 > m) { s = s * __expf(m - m2) + s2; m = m2; }
+  else s += s2 * __expf(m2 - m);
+}
+
+__device__ __forceinline__ void plp_take(float x, int i, float& m, float& s, float& bv, int& bi) {
+  if (x > bv || (x == bv && i < bi)) { bv = x; bi = i; }
+  if (x > m) { s = (m == -INFINITY ? 0.f : s * __expf(m - x)) + 1.f; m = x; }
+  else if (x > -INFINITY) s += __expf(x - m);
+}
+
+// One CTA per row. logits [Q, ld]: row q is scored against targets[q]; V real columns; out [Q, 2N+3], N in {0, 1}.
+template <typename T>
+__global__ void __launch_bounds__(kPromptLpThreads)
+prompt_logprobs_shard_kernel(const T* __restrict__ logits, int64_t ld, int V, int N,
+                             const int32_t* __restrict__ targets, float* __restrict__ out, int vocab_offset) {
+  __shared__ BlockScratch S;
+  __shared__ float s_m[32], s_s[32];
+  const int row = blockIdx.x;
+  const T* lr = logits + static_cast<size_t>(row) * ld;
+  float* o = out + static_cast<size_t>(row) * (2 * N + 3);
+  if (threadIdx.x == 0) {
+    const int local = targets[row] - vocab_offset;
+    o[2 * N + 2] = (local >= 0 && local < V) ? load_logit<T>(lr, local) : -INFINITY;
+  }
+  if (V <= 0) {   // a shard made of padding only
+    if (threadIdx.x == 0) {
+      o[2 * N] = -INFINITY;
+      o[2 * N + 1] = 0.f;
+      if (N) { o[0] = -INFINITY; o[1] = __int_as_float(kLpNoToken); }
+    }
+    return;
+  }
+  float m = -INFINITY, s = 0.f, bv = -INFINITY;
+  int bi = kLpNoToken;
+  constexpr int kVec = 16 / sizeof(T);
+  int head = 0;   // columns [0, head) go through 16-byte loads, the rest one by one
+  if ((reinterpret_cast<uintptr_t>(lr) & 15u) == 0) head = V / kVec * kVec;
+  const uint4* lv = reinterpret_cast<const uint4*>(lr);
+  for (int v = threadIdx.x; v < head / kVec; v += blockDim.x) {
+    const uint4 raw = __ldg(lv + v);
+    const T* e = reinterpret_cast<const T*>(&raw);
+    float x[kVec];
+    float vm = -INFINITY;
+#pragma unroll
+    for (int j = 0; j < kVec; ++j) {
+      x[j] = load_logit<T>(e, j);
+      vm = fmaxf(vm, x[j]);
+    }
+    const int base = v * kVec;
+#pragma unroll
+    for (int j = 0; j < kVec; ++j)
+      if (x[j] > bv) { bv = x[j]; bi = base + j; }   // ascending ids within the thread: strict > keeps the lowest
+    if (bi == kLpNoToken && vm == -INFINITY) bi = base;   // an all -inf prefix: the lowest id still wins
+    if (vm > -INFINITY) {
+      if (vm > m) { s = (m == -INFINITY ? 0.f : s * __expf(m - vm)); m = vm; }
+      float acc = 0.f;
+#pragma unroll
+      for (int j = 0; j < kVec; ++j) acc += __expf(x[j] - m);
+      s += acc;
+    }
+  }
+  for (int i = head + threadIdx.x; i < V; i += blockDim.x) plp_take(load_logit<T>(lr, i), i, m, s, bv, bi);
+  // block merge of (m, s)
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) {
+    const float m2 = __shfl_xor_sync(0xffffffffu, m, off);
+    const float s2 = __shfl_xor_sync(0xffffffffu, s, off);
+    lse_merge(m, s, m2, s2);
+  }
+  if (lane == 0) { s_m[warp] = m; s_s[warp] = s; }
+  block_argmax(bv, bi, S);   // (its __syncthreads also publish s_m / s_s)
+  if (threadIdx.x == 0) {
+    float gm = -INFINITY, gs = 0.f;
+    for (int w = 0; w < static_cast<int>(blockDim.x >> 5); ++w) lse_merge(gm, gs, s_m[w], s_s[w]);
+    o[2 * N] = gm;
+    o[2 * N + 1] = gs;
+    if (N) {
+      o[0] = bv;
+      o[1] = __int_as_float(bi == kLpNoToken ? kLpNoToken : bi + vocab_offset);
+    }
+  }
+}
+
 // set bit `token` of row `row` in the seen-token bitmask: one thread per (row, token) pair
 __global__ void mark_seen_kernel(uint32_t* seen, int seen_words, const int32_t* rows, const int32_t* tokens, int n) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -820,6 +918,24 @@ GLLM_EXPORT int gllm_logprobs_shard(const void* logits, int dtype, int64_t ld, i
       reinterpret_cast<const int32_t*>(tokens), reinterpret_cast<float*>(out), vocab_offset)
   if (dtype == 0) LP_SHARD(__nv_bfloat16); else LP_SHARD(float);
 #undef LP_SHARD
+  CUDA_CHECK_RET(cudaGetLastError());
+  return 0;
+}
+
+// Prompt log-probabilities, stage 1: `out` [Q, 2N+3] fp32 for N in {0, 1} (see prompt_logprobs_shard_kernel).
+// logits [Q, ld]: row q is scored against targets[q]; V: real vocabulary columns of this shard; vocab_offset: token id
+// of its column 0.
+GLLM_EXPORT int gllm_prompt_logprobs_shard(const void* logits, int dtype, int64_t ld, int Q, int V, int N,
+                                           const void* targets, void* out, int vocab_offset, void* stream) {
+  if (N < 0 || N > 1) return 2;
+  if (Q <= 0) return 0;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+#define PLP_SHARD(T_)                                                                                              \
+  prompt_logprobs_shard_kernel<T_><<<Q, kPromptLpThreads, 0, st>>>(                                                \
+      reinterpret_cast<const T_*>(logits), ld, V, N, reinterpret_cast<const int32_t*>(targets),                    \
+      reinterpret_cast<float*>(out), vocab_offset)
+  if (dtype == 0) PLP_SHARD(__nv_bfloat16); else PLP_SHARD(float);
+#undef PLP_SHARD
   CUDA_CHECK_RET(cudaGetLastError());
   return 0;
 }

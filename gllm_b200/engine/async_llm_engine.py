@@ -77,6 +77,8 @@ class AsyncStream:
         self.seq_id = -1
         self.aborted = False     # an abort id was sent for this request (front-end side state only)
         self.group: Optional[list] = None   # parallel sampling: the streams of all choices of the request
+        # prompt log-probs: the request's entries (None for the first token), filled before the first delta is put
+        self.prompt_logprobs: list = []
 
     def put(self, item: str):
         """Queue a text delta. With stop strings (OpenAI `stop`; not honoured by the reference) the text that could
@@ -183,20 +185,22 @@ class AsyncLLM(LLM):
     async def add_requests_async(self, raw_request, token_ids: List[int], output_len=None, ignore_eos=False,
                                  temperature=None, top_p=None, top_k=None, repetition_penalty=None,
                                  mm_contents=None, stop=None, logprobs=None, seed=None, frequency_penalty=None,
-                                 presence_penalty=None, logit_bias=None, n=None):
+                                 presence_penalty=None, logit_bias=None, n=None, prompt_logprobs=None):
         """`logprobs`: None, or N in [0, 20] — every text delta of the stream is then a `Delta` carrying the
         log-prob entries of the tokens whose text it releases (see `LLM.generate`). `seed`, `frequency_penalty`,
         `presence_penalty`, `logit_bias`: see `LLM.allocate_seq` (ValueError when out of range).
         Returns the request's `AsyncStream`; with `n` given (parallel sampling, see `LLM.allocate_choices`) a list of
-        one stream per choice, in choice order. A stop string ends only its own choice."""
+        one stream per choice, in choice order. A stop string ends only its own choice. `prompt_logprobs`: see
+        `LLM.generate`; every stream's `prompt_logprobs` is the request's list, complete before its first delta."""
         seqs = self.allocate_choices(token_ids, n, output_len, ignore_eos, temperature, top_p, top_k,
                                      repetition_penalty, mm_contents, logprobs, seed, frequency_penalty,
-                                     presence_penalty, logit_bias)
+                                     presence_penalty, logit_bias, prompt_logprobs)
         streams = []
         for seq in seqs:
             stream = AsyncStream(raw_request, stop, logprobs=logprobs is not None)
             stream.prompt_tokens = len(token_ids)
             stream.seq_id = seq.seq_id
+            stream.prompt_logprobs = seq.prompt_logprobs
             self.async_streams[seq.seq_id] = stream
             streams.append(stream)
         if len(streams) > 1:

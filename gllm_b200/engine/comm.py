@@ -34,6 +34,7 @@ class IPCPackage:
     act_schedule_ids: list = field(default_factory=list)  # driver -> front-end
     next_tokens: list = field(default_factory=list)
     next_logprobs: Optional[list] = None   # aligned with next_tokens when some request asked for log-probs
+    prompt_logprobs: Optional[dict] = None  # seq id -> its next prompt log-prob entries, in prompt order
     free_ids: list = field(default_factory=list)
     control_cmd: Optional[tuple] = None
     stats: Optional[dict] = None
@@ -208,9 +209,12 @@ class Comm:
         return "batch", self._decode_batch(buf[1:])
 
     # output rank -> driver -----------------------------------------------------------------------
-    def send_tokens(self, batch_id: int, tokens: List[int], logprobs: Optional[list] = None):
-        """`logprobs`: None, or one entry per token (see StepResult.logprobs_list)."""
-        self.tok_out.send(pickle.dumps((batch_id, tokens, logprobs), protocol=pickle.HIGHEST_PROTOCOL))
+    def send_tokens(self, batch_id: int, tokens: List[int], logprobs: Optional[list] = None,
+                    prompt_logprobs: Optional[list] = None):
+        """`logprobs`: None, or one entry per token (see StepResult.logprobs_list); `prompt_logprobs`: None, or one
+        entry per prompt row (see StepResult.prompt_logprobs_list)."""
+        self.tok_out.send(pickle.dumps((batch_id, tokens, logprobs, prompt_logprobs),
+                                       protocol=pickle.HIGHEST_PROTOCOL))
 
     def recv_tokens(self):
         out = []

@@ -52,6 +52,19 @@ def check_n(n, max_running_seqs: int, multimodal: bool = False) -> int:
     return n
 
 
+def check_prompt_logprobs(prompt_logprobs, multimodal: bool = False) -> int:
+    """Validate `prompt_logprobs` -> N, or -1 for None (no prompt log-probs). Raises ValueError: N must be an integer
+    in [0, MAX_LOGPROBS]; multimodal input is refused (image placeholder tokens make no sensible targets)."""
+    if prompt_logprobs is None:
+        return -1
+    if isinstance(prompt_logprobs, bool) or not isinstance(prompt_logprobs, int) or \
+            not 0 <= prompt_logprobs <= MAX_LOGPROBS:
+        raise ValueError(f"prompt_logprobs must be an integer in [0, {MAX_LOGPROBS}]")
+    if multimodal:
+        raise ValueError("prompt_logprobs is not supported with multimodal input")
+    return prompt_logprobs
+
+
 def choice_seed(seed: Optional[int], i: int) -> Optional[int]:
     """Seed of choice i of a request seeded with `seed`: seed + i, wrapped to a signed 64-bit int."""
     if seed is None:
@@ -277,14 +290,16 @@ class LLM:
 
     def allocate_seq(self, token_ids: List[int], output_len=None, ignore_eos=False, temperature=None, top_p=None,
                      top_k=None, repetition_penalty=None, mm_contents=None, logprobs=None, seed=None,
-                     frequency_penalty=None, presence_penalty=None, logit_bias=None) -> Sequence:
+                     frequency_penalty=None, presence_penalty=None, logit_bias=None, prompt_logprobs=None) -> Sequence:
         """Defaults: temperature/top_p/repetition_penalty from generation_config, top_k = 1
         (greedy) unless given (reference: gllm/llm_engine.py:305-337). `logprobs`: None (no log-probs) or the number
         N in [0, MAX_LOGPROBS] of most likely tokens to report next to every generated token's log-prob.
+        `prompt_logprobs`: likewise for every prompt token after the first (`Sequence.prompt_logprobs`).
         `seed`, `frequency_penalty`, `presence_penalty`, `logit_bias`: OpenAI semantics, validated by
         `check_sampling_params` (see entrypoints/protocol.py for the formula)."""
         if logprobs is not None and not 0 <= int(logprobs) <= MAX_LOGPROBS:
             raise ValueError(f"logprobs must be in [0, {MAX_LOGPROBS}]")
+        plp = check_prompt_logprobs(prompt_logprobs, bool(mm_contents))
         seed, frequency_penalty, presence_penalty, logit_bias = check_sampling_params(
             seed, frequency_penalty, presence_penalty, logit_bias, self.loader.config.get("vocab_size"))
         if len(token_ids) == 0:
@@ -300,7 +315,7 @@ class LLM:
                        1 if top_k is None else top_k,
                        self.default_repetition_penalty if repetition_penalty is None else repetition_penalty,
                        mm_contents, -1 if logprobs is None else int(logprobs), seed, frequency_penalty,
-                       presence_penalty, logit_bias)
+                       presence_penalty, logit_bias, plp)
         if output_len is None:
             seq.output_len = min(4096, self.model_max_length - len(token_ids))
         if mm_contents:
@@ -311,11 +326,13 @@ class LLM:
 
     def allocate_choices(self, token_ids: List[int], n=None, output_len=None, ignore_eos=False, temperature=None,
                          top_p=None, top_k=None, repetition_penalty=None, mm_contents=None, logprobs=None, seed=None,
-                         frequency_penalty=None, presence_penalty=None, logit_bias=None) -> List[Sequence]:
+                         frequency_penalty=None, presence_penalty=None, logit_bias=None,
+                         prompt_logprobs=None) -> List[Sequence]:
         """The `n` choices of one request (parallel sampling; see `check_n`): choice 0 is the request as `allocate_seq`
         makes it, choices 1..n-1 are its forks (`Sequence.forks`): the prompt is prefilled once and every choice draws
         its first token from the same logits row, then continues on its own. With a seed, choice i uses seed + i.
-        Only choice 0 goes to `add_requests`; the forks travel with it."""
+        Only choice 0 goes to `add_requests`; the forks travel with it. The prompt's log-probs are computed once: every
+        choice holds the same `prompt_logprobs` list."""
         k = check_n(n, self.cfg.max_running_seqs, bool(mm_contents))
         seqs = []
         try:
@@ -323,13 +340,15 @@ class LLM:
                 seqs.append(self.allocate_seq(token_ids, output_len, ignore_eos, temperature, top_p, top_k,
                                               repetition_penalty, mm_contents, logprobs,
                                               choice_seed(seed, i) if i else seed, frequency_penalty, presence_penalty,
-                                              logit_bias))
+                                              logit_bias, prompt_logprobs))
         except Exception:
             with self._inbox_lock:
                 for s in seqs:
                     self.id_allocator.free(s.seq_id)
             raise
         seqs[0].forks = seqs[1:]
+        for s in seqs[1:]:
+            s.prompt_logprobs = seqs[0].prompt_logprobs
         return seqs
 
     # The three inboxes below are filled from request handlers (event-loop thread of the API server) while the
@@ -382,6 +401,10 @@ class LLM:
         now = time.time()
         inproc = self.worker is not None
         lps = pkg.next_logprobs
+        for sid, entries in (pkg.prompt_logprobs or {}).items():
+            seq = self.running_maps.get(sid)
+            if seq is not None:
+                seq.prompt_logprobs.extend(entries)     # (shared by the choices of a request)
         for i, (sid, tok) in enumerate(zip(pkg.act_schedule_ids, pkg.next_tokens)):
             seq = self.running_maps.get(sid)
             if seq is None:
@@ -424,7 +447,8 @@ class LLM:
                  output_lens: Optional[List[int]] = None, temperature=None, top_p=None, top_k=None,
                  repetition_penalty=None, ignore_eos: bool = False, progress: bool = False,
                  mm_contents: Optional[List[Optional[dict]]] = None, logprobs=None, seed=None,
-                 frequency_penalty=None, presence_penalty=None, logit_bias=None, n=None) -> List[Sequence]:
+                 frequency_penalty=None, presence_penalty=None, logit_bias=None, n=None,
+                 prompt_logprobs=None) -> List[Sequence]:
         """Batch generation; returns the finished `Sequence`s in request order with `.prompt`,
         `.output`, `.token_ids` (reference: gllm/llm_engine.py:343-378). `mm_contents[i]` (VL models) is
         the processor output of request i: pixel_values / image_grid_thw [/ pixel_values_videos ...].
@@ -434,7 +458,12 @@ class LLM:
         `seed`, `frequency_penalty`, `presence_penalty`, `logit_bias` ({token id: bias}): OpenAI sampling parameters,
         one value or one per request like the others (a dict is one value for all requests).
         `n` (parallel sampling, one value or one per request): request j gives n_j choices, returned consecutively in
-        choice order; the prompt is prefilled once (see `allocate_choices`)."""
+        choice order; the prompt is prefilled once (see `allocate_choices`).
+        `prompt_logprobs` (None or N in [0, 20], one value or one per request): `.prompt_logprobs` gets one entry per
+        prompt token — None for the first, then (its log-prob given the tokens before it, [(token, log-prob) of the N
+        most likely tokens at that position]), under the same distribution as `logprobs`; [] when not asked. Not
+        available with multimodal input. Such a request takes no prefix-cache hits (it needs every prompt position's
+        hidden state); it still publishes its pages for later requests."""
         if self.worker is not None and self.worker.rank != 0:
             return self._serve_until_stop()
         if tokens is None:
@@ -452,7 +481,7 @@ class LLM:
                                             pick(repetition_penalty),
                                             mm_contents[i] if mm_contents is not None else None, pick(logprobs),
                                             pick(seed), pick(frequency_penalty), pick(presence_penalty),
-                                            pick(logit_bias))
+                                            pick(logit_bias), pick(prompt_logprobs))
             heads.append(choices[0])
             seqs.extend(choices)
         n = len(seqs)

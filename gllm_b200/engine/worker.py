@@ -117,7 +117,7 @@ class Worker(ProfilerMixin):
 
     def _to_frontend(self, out: SchedulerOutput):
         pkg = IPCPackage(act_schedule_ids=out.act_schedule_ids, next_tokens=out.next_tokens,
-                         next_logprobs=out.next_logprobs, free_ids=out.free_ids)
+                         next_logprobs=out.next_logprobs, free_ids=out.free_ids, prompt_logprobs=out.prompt_logprobs)
         if self.scheduler is not None:
             pkg.stats = dict(self.scheduler.last_stats)
             pkg.stats.update(self.phase_stats)
@@ -137,8 +137,8 @@ class Worker(ProfilerMixin):
         did |= self._recv_frontend()
         # tokens coming back from the output rank (pp > 1 or tp-only with output rank != 0)
         if self.comm is not None:
-            for batch_id, toks, lps in self.comm.recv_tokens():
-                sch.add_next_tokens(toks, lps)
+            for batch_id, toks, lps, plp in self.comm.recv_tokens():
+                sch.add_next_tokens(toks, lps, plp)
                 did = True
         if self.cfg.async_schedule and len(self.pending) == 1:
             # async scheduling: queue the NEXT decode step behind the one still running on the GPU, before its
@@ -158,7 +158,7 @@ class Worker(ProfilerMixin):
             self.phase_stats[phase + "_step_seconds"] += time.perf_counter() - t0
             self.phase_stats[phase + "_step_count"] += 1
             self.phase_stats[phase + "_step_tokens"] += ntok
-            sch.add_next_tokens(res.tokens_list(), res.logprobs_list())
+            sch.add_next_tokens(res.tokens_list(), res.logprobs_list(), res.prompt_logprobs_list())
             did = True
         while True:
             out = sch.process_output()
@@ -265,7 +265,8 @@ class Worker(ProfilerMixin):
         res = self.runner.step(batch, hidden, residual, recv_tiles=tiles)
         if ps.is_last_pp_rank():
             if ps.is_output_rank():
-                self.comm.send_tokens(batch.batch_id, res.tokens_list(), res.logprobs_list())
+                self.comm.send_tokens(batch.batch_id, res.tokens_list(), res.logprobs_list(),
+                                      res.prompt_logprobs_list())
         else:
             self._pp_send(res)
         return True

@@ -61,6 +61,19 @@ def _validate_logprobs(request, chat: bool):
     return None
 
 
+def _validate_prompt_logprobs(request):
+    """`prompt_logprobs` sets the N of the echoed prompt's entries: without `echo` and `logprobs` there is nowhere to
+    report them, so it is refused rather than ignored."""
+    from gllm_b200.engine.llm_engine import check_prompt_logprobs
+    try:
+        check_prompt_logprobs(request.prompt_logprobs)
+    except ValueError as e:
+        return str(e)
+    if request.prompt_logprobs is not None and not (request.echo and request.logprobs is not None):
+        return "prompt_logprobs needs echo: true and logprobs"
+    return None
+
+
 def _check_params(request, multimodal: bool = False):
     """-> (error message or None, kwargs of the OpenAI sampling parameters for add_requests_async). `n` is passed
     only when it is above 1, so an n = 1 request takes exactly the path it took before parallel sampling."""
@@ -95,16 +108,32 @@ def _chat_logprobs(entries):
 
 def _completion_logprobs(entries, offset: int = 0):
     """Legacy completions shape {tokens, token_logprobs, top_logprobs: [{token: logprob}], text_offset}; `offset` is
-    the text offset of the first entry. Returns (logprobs, offset after the last entry)."""
+    the text offset of the first entry. Returns (logprobs, offset after the last entry). An entry (tok, None, None) is
+    the first prompt token, which nothing predicts: null log-prob and null alternatives."""
     out = {"tokens": [], "token_logprobs": [], "top_logprobs": [], "text_offset": []}
     for tok, lp, top in entries:
         s = _token_str(tok)
         out["tokens"].append(s)
-        out["token_logprobs"].append(_lp_num(lp))
-        out["top_logprobs"].append({_token_str(t): _lp_num(v) for t, v in top})
+        out["token_logprobs"].append(None if lp is None else _lp_num(lp))
+        out["top_logprobs"].append(None if top is None else {_token_str(t): _lp_num(v) for t, v in top})
         out["text_offset"].append(offset)
         offset += len(s)
     return out, offset
+
+
+def _prompt_entries(token_ids, prompt_logprobs):
+    """Completion-shaped entries (token, log-prob, alternatives) of the prompt: the first token has none."""
+    return [(token_ids[0], None, None)] + [(t, lp, top) for t, (lp, top) in zip(token_ids[1:], prompt_logprobs[1:])]
+
+
+def _prompt_text(prompt, token_ids) -> str:
+    if isinstance(prompt, str):
+        return prompt
+    if isinstance(prompt, list) and prompt and isinstance(prompt[0], str):
+        return prompt[0]
+    if llm.tokenizer is not None:
+        return llm.tokenizer.decode(token_ids)
+    return "".join(_token_str(t) for t in token_ids)
 
 
 def _validate(token_ids, output_len, vocab_size=None):
@@ -202,24 +231,48 @@ async def chat_completion_stream_generator(streams, request):
     yield "data: [DONE]\n\n"
 
 
-async def completion_generator(streams, request) -> CompletionResponse:
+async def completion_generator(streams, request, echo=None) -> CompletionResponse:
+    """`echo`: None, or (prompt text, prompt token ids) to put in front of every choice."""
     texts = await asyncio.gather(*(llm.collect(st) for st in streams))
     choices = []
     for i, (st, text) in enumerate(zip(streams, texts)):
-        choice = CompletionResponseChoice(index=i, text=text, finish_reason=st.finish_reason)
+        gen = st.logprobs_out
+        if echo is not None and request.max_tokens == 0:
+            text, gen, st.completion_tokens, st.finish_reason = "", [], 0, "length"   # the sampled token is dropped
+        choice = CompletionResponseChoice(index=i, text=text if echo is None else echo[0] + text,
+                                          finish_reason=st.finish_reason)
         if st.want_logprobs:
-            choice.logprobs = _completion_logprobs(st.logprobs_out)[0]
+            pre = _prompt_entries(echo[1], st.prompt_logprobs) if echo is not None else []
+            choice.logprobs = _completion_logprobs(pre + gen)[0]
         choices.append(choice)
     return CompletionResponse(choices=choices, model=request.model, usage=_usage(streams))
 
 
-async def completion_stream_generator(streams, request):
+async def completion_stream_generator(streams, request, echo=None):
+    """`echo`: None, or (prompt text, prompt token ids): the first chunk of each choice carries the prompt text (and
+    its log-prob entries), before any generated text."""
     rid = None
     offset = [0] * len(streams)
     left = len(streams)
+    echoed = [echo is None] * len(streams)
+    drop = echo is not None and request.max_tokens == 0     # the engine's one sampled token is not part of the answer
     try:
         async for i, delta in _merge(streams):
             st = streams[i]
+            if not echoed[i]:
+                echoed[i] = True
+                chunk = CompletionStreamResponse(choices=[CompletionResponseStreamChoice(index=i, text=echo[0])],
+                                                 model=request.model)
+                if st.want_logprobs:
+                    chunk.choices[0].logprobs, offset[i] = _completion_logprobs(
+                        _prompt_entries(echo[1], st.prompt_logprobs), offset[i])
+                rid = rid or chunk.id
+                chunk.id = rid
+                yield f"data: {chunk.model_dump_json(exclude_unset=False)}\n\n"
+            if drop:
+                if delta is not None:
+                    continue
+                st.completion_tokens, st.finish_reason = 0, "length"
             if delta is None:
                 left -= 1
                 chunk = CompletionStreamResponse(
@@ -338,20 +391,28 @@ def build_app(engine):
         except Exception as e:  # noqa: BLE001
             return _error(f"cannot encode prompt: {e}")
         bad, params = _check_params(request)
+        # `max_tokens: 0` (scoring the prompt alone) is served with echo: one token is sampled and dropped
+        max_tokens = 1 if request.echo and request.max_tokens == 0 else request.max_tokens
         bad = bad or _validate_sampling(request) or _validate_logprobs(request, chat=False) or \
-            _validate(token_ids, request.max_tokens, llm.loader.config.get("vocab_size"))
+            _validate_prompt_logprobs(request) or \
+            _validate(token_ids, max_tokens, llm.loader.config.get("vocab_size"))
         if bad:
             return _error(bad)
         if llm.failed:
             return _error(f"engine is down: {llm.failed}", HTTPStatus.INTERNAL_SERVER_ERROR)
-        stream = await llm.add_requests_async(raw_request, token_ids, request.max_tokens, request.ignore_eos,
+        if request.echo and request.logprobs is not None:
+            params["prompt_logprobs"] = request.logprobs if request.prompt_logprobs is None else \
+                request.prompt_logprobs
+        stream = await llm.add_requests_async(raw_request, token_ids, max_tokens, request.ignore_eos,
                                               request.temperature, request.top_p, request.top_k,
                                               request.repetition_penalty, stop=request.stop,
                                               logprobs=request.logprobs, **params)
         streams = stream if "n" in params else [stream]
+        echo = (await _in_thread(_prompt_text, request.prompt, token_ids), token_ids) if request.echo else None
         if request.stream:
-            return StreamingResponse(completion_stream_generator(streams, request), media_type="text/event-stream")
-        return JSONResponse(content=(await completion_generator(streams, request)).model_dump())
+            return StreamingResponse(completion_stream_generator(streams, request, echo),
+                                     media_type="text/event-stream")
+        return JSONResponse(content=(await completion_generator(streams, request, echo)).model_dump())
 
     @app.post("/tokenize")
     async def tokenize(request: TokenizeRequest):

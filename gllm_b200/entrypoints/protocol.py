@@ -9,8 +9,7 @@ distribution: log_softmax in fp32 of the logits the LM head produced, over the r
 penalty, temperature, top-k and top-p. So they do not depend on the sampling parameters, and the sampled token's
 log-prob is reported under that distribution even when it was drawn with a temperature or a filter. Every generated
 token gets its log-prob and the N most likely tokens (0 <= N <= 20), ordered by logit, ties to the lower token id; for
-a greedy request the first of them is the sampled token when it uses no penalty or bias. Prompt tokens get none (`echo`
-is ignored). Token strings are `tokenizer.decode([id])` (`bytes`: its UTF-8 encoding), or "token_id:<id>" without a
+a greedy request the first of them is the sampled token when it uses no penalty or bias. Token strings are `tokenizer.decode([id])` (`bytes`: its UTF-8 encoding), or "token_id:<id>" without a
 tokenizer. A log-prob of -inf is reported as -9999.0. Out-of-range `top_logprobs` / `logprobs`, or `top_logprobs > 0` without `logprobs`, is a 400.
 
 `frequency_penalty`, `presence_penalty` and `logit_bias` follow OpenAI's formula. For a generated token, with x the
@@ -27,6 +26,17 @@ it draws the same token whatever the batch, its row in it, the engine's step cou
 or the tensor-parallel degree; without a seed the draw comes from the engine's own stream. A 400 answers: a penalty
 outside [-2, 2] or not finite; a logit_bias key that is not an int in [0, vocab_size), a value outside [-100, 100] or
 not finite, or more than 1024 entries (this engine's own cap); a seed that does not fit a signed 64-bit int.
+
+Completions `echo: true` puts the prompt text in front of each choice's `text` (a token-id prompt is decoded). With
+`logprobs: N` as well, `tokens` / `token_logprobs` / `top_logprobs` / `text_offset` start with the prompt's entries,
+under the same distribution and with the same N (`prompt_logprobs: M` sets another N for the prompt; it is a 400
+without `echo: true` and `logprobs`, which are where the entries are reported): the first prompt
+token has `token_logprobs[0] = null` and `top_logprobs[0] = null`, and `text_offset` runs from 0 across prompt and
+completion. When streaming, the first chunk of each choice carries the echoed prompt and its entries. `max_tokens: 0`
+is accepted only with `echo: true`: the response is the echoed prompt (and its entries) with `finish_reason: "length"`
+and `usage.completion_tokens = 0`; the engine still samples one token internally and drops it. A request with prompt
+log-probs takes no prefix-cache hits. `prompt_logprobs` outside [0, 20] is a 400. Chat completions have no prompt
+log-probs.
 
 `n` asks for n independent choices of one request (parallel sampling). The prompt is prefilled once, its full KV
 pages are shared by the choices and its partial last page is copied on the device; every choice draws its first token
@@ -144,6 +154,7 @@ class CompletionRequest(_SamplingMixin):
     max_tokens: Optional[int] = 16
     echo: Optional[bool] = False
     logprobs: Optional[int] = None
+    prompt_logprobs: Optional[int] = None
     suffix: Optional[str] = None
     best_of: Optional[int] = None
 

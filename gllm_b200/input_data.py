@@ -81,6 +81,11 @@ class BatchArrays:
     # parallel sampling: (src, dst) KV pages every rank copies for its own layers right after this batch's forward
     # (the partial last prompt page of a request that fans out into several choices); None when there is none
     kv_copy: Optional[np.ndarray] = None     # int32 [C, 2]
+    # prompt log-probabilities: rows (in the batch's token order) whose logits score the next prompt token, that
+    # token, and the largest N any of them asks for; None / -1 when no row asks
+    plp_rows: Optional[np.ndarray] = None    # int32 [Q]
+    plp_targets: Optional[np.ndarray] = None  # int32 [Q]
+    plp_n: int = -1
     emit_ids: Optional[list] = None  # driver-local: sequence id per EMITTING entry (order of the sampler output)
     seq_ids: Optional[list] = None  # driver-local: sequence id per row (incremental decode batches); not sent
     pt_gens: Optional[list] = None  # driver-local: Sequence.pt_gen per row when the block table rows were written
@@ -101,12 +106,14 @@ class BatchArrays:
                  "logits_idx", "emit_seq", "temperature", "top_k", "top_p", "rep_penalty", "state_slot"]
         opt = ["seen_rows", "seen_tokens", "clear_slots", "feed_src", "logprobs_n", "freq_pen", "pres_pen",
                "bias_slot", "rb_slots", "rb_pen", "rb_lb_off", "rb_lb_ids", "rb_lb_vals", "rb_out_off", "rb_out_toks",
-               "seed", "seed_pos", "kv_copy"]
+               "seed", "seed_pos", "kv_copy", "plp_rows", "plp_targets"]
         scalars = (self.num_decode_seqs, self.num_seqs, self.num_tokens, self.max_q_len, self.max_seq_len,
                    self.all_greedy, self.need_penalty, self.batch_id)
         if self.need_bias:      # (only then: a batch without the feature sends the header it always sent)
             scalars += (True,)
         hdr = {"scalars": scalars, "arrays": [], "mm": self.mm}
+        if self.plp_rows is not None:
+            hdr["plp_n"] = self.plp_n
         parts, off = [], 0
         for n in names + opt:
             a = getattr(self, n)
@@ -133,7 +140,7 @@ class BatchArrays:
         s = hdr["scalars"]
         return BatchArrays(**kw, num_decode_seqs=s[0], num_seqs=s[1], num_tokens=s[2], max_q_len=s[3],
                            max_seq_len=s[4], all_greedy=s[5], need_penalty=s[6], batch_id=s[7], mm=hdr.get("mm"),
-                           need_bias=len(s) > 8 and s[8])
+                           need_bias=len(s) > 8 and s[8], plp_n=hdr.get("plp_n", -1))
 
 
 def _page_array(seq) -> np.ndarray:
@@ -268,6 +275,7 @@ def build_batch(entries, page_size: int, vocab_size: int, batch_id: int = 0, mro
     rb_slots, rb_pen, rb_lb_ids, rb_lb_vals, rb_out_toks, rb_lb_off, rb_out_off = [], [], [], [], [], [0], [0]
     seeds, seed_pos, want_seed = [], [], False
     emit_rows, fork_rows, kv_copy = [], [], []   # (entry, logits row, sequence, end of its known tokens)
+    plp_rows, plp_targets, plp_n = [], [], -1
     for i, e in enumerate(entries):
         seq = e.seq
         pt = _page_array(seq)
@@ -292,6 +300,17 @@ def build_batch(entries, page_size: int, vocab_size: int, batch_id: int = 0, mro
             else:
                 positions[a:z] = pos
             slots[a:z] = pt[pos // page_size] * page_size + pos % page_size
+        if seq.prompt_logprobs_n >= 0 and not e.is_decode:
+            # prompt positions [lo, hi) score tokens lo + 1 .. hi; position P - 1 is the sampled row. The cursor makes
+            # every position go out once, whatever the chunking or a recompute after preemption.
+            lo, hi = max(s0, seq.plp_cursor), min(s0 + e.n, seq.prompt_len - 1)
+            if hi > lo:
+                assert lo == seq.plp_cursor, (seq.seq_id, s0, seq.plp_cursor)
+                plp_rows.append(np.arange(a + lo - s0, a + hi - s0, dtype=np.int32))
+                plp_targets.append(np.asarray(seq.token_ids[lo + 1:hi + 1], dtype=np.int32))
+                plp_n = max(plp_n, seq.prompt_logprobs_n)
+                seq.plp_cursor = hi
+                e.plp = hi - lo
         if e.emits:
             emit_rows.append((i, z - 1, seq, s0 + e.n))
             for sib in e.forks or ():        # parallel sampling: the other choices draw from the same logits row
@@ -373,6 +392,8 @@ def build_batch(entries, page_size: int, vocab_size: int, batch_id: int = 0, mro
         seed=np.asarray(seeds, dtype=np.int64) if want_seed else None,
         seed_pos=np.asarray(seed_pos, dtype=np.int32) if want_seed else None,
         kv_copy=np.asarray(kv_copy, dtype=np.int32).reshape(-1, 2) if kv_copy else None,
+        plp_rows=np.concatenate(plp_rows) if plp_rows else None,
+        plp_targets=np.concatenate(plp_targets) if plp_rows else None, plp_n=plp_n,
         **(_bias_fields(freq_pen, pres_pen, bias_slot, rb_slots, rb_pen, rb_lb_off, rb_lb_ids, rb_lb_vals, rb_out_off,
                         rb_out_toks) if need_bias else {}),
         seq_ids=[e.seq.seq_id for e in entries] if n_dec == b else None,
@@ -421,6 +442,8 @@ class InputData:
         self._bias_slot = buf((max_seqs,), i32)
         self._seed = buf((max_seqs,), torch.int64)
         self._seed_pos = buf((max_seqs,), i32)
+        self._buf = buf
+        self._plp = None   # (rows, targets) of prompt log-prob rows: allocated by the first batch that has them
         self.need_tok_seq = False  # MLA attention wants token -> sequence for mixed / prefill batches
         self.batch: Optional[BatchArrays] = None
         self.num_tokens = self.num_seqs = self.num_decode_seqs = self.num_emit = 0
@@ -465,6 +488,11 @@ class InputData:
             self._put(self._tok_seq, np.repeat(np.arange(batch.num_seqs, dtype=np.int32), np.diff(qsl)))
         if batch.feed_src is not None:
             self._put(self._feed, batch.feed_src)
+        if batch.plp_rows is not None:
+            if self._plp is None:
+                self._plp = (self._buf((self.max_tokens,), torch.int32), self._buf((self.max_tokens,), torch.int32))
+            self._put(self._plp[0], batch.plp_rows)
+            self._put(self._plp[1], batch.plp_targets)
         self._put(self._block_table, batch.block_table)
         self._put(self._seq_lens, batch.seq_lens)
         self._put(self._qsl, batch.query_start_loc)
@@ -576,6 +604,12 @@ class InputData:
         return self._bias_slot[1][: self.num_emit] if self.batch is not None and self.batch.need_bias else None
 
     @property
+    def plp(self):
+        """(int32 rows [Q], int32 targets [Q]) of the batch's prompt log-prob rows on the device."""
+        q = self.batch.plp_rows.shape[0]
+        return self._plp[0][1][:q], self._plp[1][1][:q]
+
+    @property
     def seeds(self):
         """(int64 seeds [E], int32 positions [E]) of a batch with seeded rows, else (None, None)."""
         if self.batch is None or self.batch.seed is None:
@@ -590,7 +624,7 @@ class InputData:
         for a in (b.tokens, b.positions, b.slot_mapping, b.block_table, b.seq_lens, b.query_start_loc,
                   b.logits_idx, b.temperature, b.top_k, b.top_p, b.rep_penalty, b.state_slot):
             tot += a.nbytes
-        for a in (b.freq_pen, b.pres_pen, b.bias_slot, b.seed, b.seed_pos):
+        for a in (b.freq_pen, b.pres_pen, b.bias_slot, b.seed, b.seed_pos, b.plp_rows, b.plp_targets):
             if a is not None:
                 tot += a.nbytes
         return tot

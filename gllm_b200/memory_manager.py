@@ -158,6 +158,8 @@ class PrefixMemoryManager(MemoryManager):
             # never serve the *whole* prompt from cache: the last token must be computed to get logits
             if full * ps == n_tok:
                 full -= 1
+            if seq.plp_pending:
+                full = 0     # prompt log-probs need the hidden state of every prompt position: no hits
             self._extend_hashes(seq, max(full, 0))
             for i in range(max(full, 0)):
                 page = self.hash2page.get(seq.page_hashes[i])

@@ -42,6 +42,10 @@ class StepResult:
     logprobs: Optional[torch.Tensor] = None
     logprobs_host: Optional[torch.Tensor] = None
     logprobs_n: Optional[np.ndarray] = None
+    # prompt log-probabilities (only when the batch has prompt rows): fp32 [Q, 1 + 2N] in the batch's prompt-row order
+    # and its pinned copy (same event)
+    prompt_logprobs: Optional[torch.Tensor] = None
+    prompt_logprobs_host: Optional[torch.Tensor] = None
 
     def tokens_list(self) -> List[int]:
         if self.tokens is None:
@@ -67,10 +71,29 @@ class StepResult:
             if n < 0:
                 out.append(None)
                 continue
-            top = [(int(ids[j, 1 + 2 * i]), float(vals[j, 2 + 2 * i])) for i in range(n) if ids[j, 1 + 2 * i] >= 0]
-            out.append((float(vals[j, 0]), top))
+            out.append(_entry(vals, ids, j, n))
             j += 1
         return out
+
+    def prompt_logprobs_list(self) -> Optional[list]:
+        """None when the batch had no prompt rows; else per prompt row (target token's log-prob, [(token, log-prob),
+        ...] with the batch's N most likely tokens, largest first)."""
+        lp = self.prompt_logprobs
+        if lp is None:
+            return None
+        if self.event is not None:
+            self.event.synchronize()
+            lp = self.prompt_logprobs_host[: lp.numel()].view(lp.shape)
+        vals = lp.cpu().numpy()
+        ids = vals.view(np.int32)
+        n = (lp.shape[1] - 1) // 2
+        return [_entry(vals, ids, j, n) for j in range(lp.shape[0])]
+
+
+def _entry(vals: np.ndarray, ids: np.ndarray, j: int, n: int):
+    """(chosen log-prob, [(token, log-prob)] of the n most likely) from row j of a logprobs_final result."""
+    top = [(int(ids[j, 1 + 2 * i]), float(vals[j, 2 + 2 * i])) for i in range(n) if ids[j, 1 + 2 * i] >= 0]
+    return float(vals[j, 0]), top
 
 
 class ModelRunner:
@@ -150,6 +173,8 @@ class ModelRunner:
             self._host_flip = 0
             self.tokens_host = self._tokens_host2[0]
             self._lp_host2 = None        # pinned log-prob result buffers, allocated on the first request that asks
+            self._plp_host2 = None       # the same for prompt log-probs
+        self._plp = None                 # this step's prompt log-prob result, from the forward to the sampling
         logger.info("model loaded in %.1fs", time.time() - t0)
         self.profile_run()
         self.num_pages = self.compute_num_pages()
@@ -217,8 +242,23 @@ class ModelRunner:
             h, r = self.model(inp, kv, self.tpc, hidden, residual)
         if ps.is_last_pp_rank():
             vp = self.sampler.vocab_parallel
+            h = self.tpc.materialize(h)
+            if not all_rows and inp.batch is not None and inp.batch.plp_rows is not None:
+                # before the sampled rows' logits: the step's logits footprint stays within one [R, Vp/tp] tile or
+                # the [E, Vp/tp] logits, both covered by the profile run
+                self._plp = self.sampler.prompt_logprobs(inp.batch, h, self.model.lm_head, self.plp_tile_rows())
             return self.model.compute_logits(inp, h, self.tpc, all_rows=all_rows, local=vp), None
         return h, r
+
+    # prompt rows per LM-head tile. Measured on H100 at V = 151936, tp 1 and 2 (benchmarks/prompt_logprobs_bench.py,
+    # README): 256-row tiles cost half as much per row as 128-row ones in the GEMM, and the one-pass records kernel
+    # still reads a tile right after its GEMM at 1.5-3.5 TB/s (tp 2 - tp 1; partly from L2). Capped by
+    # max_running_seqs, so a tile is never wider than the [max_running_seqs, Vp/tp] logits the profile run
+    # materialises.
+    PLP_TILE_ROWS = 256
+
+    def plp_tile_rows(self) -> int:
+        return max(1, min(self.PLP_TILE_ROWS, self.max_running_seqs))
 
     def capture_graphs(self):
         """Decode-only batches replay a CUDA graph per power-of-two bucket (forward -> logits)."""
@@ -330,6 +370,7 @@ class ModelRunner:
                     w.wait()
             recv_tiles = None
         if bucket is not None:
+            assert batch.plp_rows is None, "a decode-only batch carries no prompt rows"
             g, splits = self.graphs[bucket]
             inp.pad_for_graph(bucket, (self.num_pages - 1) * self.page_size, self.num_pages - 1)
             g.replay()
@@ -348,15 +389,19 @@ class ModelRunner:
 
     def _sample(self, batch: BatchArrays, logits: torch.Tensor) -> StepResult:
         e = logits.shape[0]
+        plp, self._plp = self._plp, None
         if e == 0:
-            return StepResult(tokens=self.tokens_out[:0], num_emit=0)
+            if plp is None:
+                return StepResult(tokens=self.tokens_out[:0], num_emit=0)
+            return self._finish_sample(self.tokens_out[:0], 0, None, plp)
         if self.keep_logits:
             full = self.tpc.gather_logits(logits, self.spec.vocab_size) if self.sampler.vocab_parallel else logits
             self.logit_log.append((list(batch.emit_ids or []), full[:e, : self.spec.vocab_size].float().cpu()))
         toks, logprobs = self.sampler.sample(batch, logits)
-        return self._finish_sample(toks, e, logprobs)
+        return self._finish_sample(toks, e, logprobs, plp)
 
-    def _finish_sample(self, toks: torch.Tensor, e: int, logprobs: Optional[torch.Tensor] = None) -> StepResult:
+    def _finish_sample(self, toks: torch.Tensor, e: int, logprobs: Optional[torch.Tensor] = None,
+                       plp: Optional[torch.Tensor] = None) -> StepResult:
         self.tokens_out[:e].copy_(toks)
         # (CPU: no async D2H copy — snapshot the values, a lookahead step may overwrite tokens_out before the
         # scheduler reads them)
@@ -364,6 +409,7 @@ class ModelRunner:
                          num_emit=e)
         if logprobs is not None:
             res.logprobs, res.logprobs_n = logprobs, self.input_data.batch.logprobs_n[:e]
+        res.prompt_logprobs = plp
         if self.device.type == "cuda":
             self._host_flip ^= 1
             self.tokens_host = self._tokens_host2[self._host_flip]
@@ -380,6 +426,15 @@ class ModelRunner:
                 host[: logprobs.numel()].copy_(logprobs.view(-1), non_blocking=True)
                 res.logprobs_host = host
                 self.stats["d2h_bytes"] += 4 * logprobs.numel()
+            if plp is not None:
+                if self._plp_host2 is None:
+                    from gllm_b200.ops.sm100 import MAX_LOGPROBS
+                    size = self.max_num_batched_tokens * (1 + 2 * MAX_LOGPROBS)
+                    self._plp_host2 = [torch.zeros(size, dtype=torch.float32, pin_memory=True) for _ in range(2)]
+                host = self._plp_host2[self._host_flip]
+                host[: plp.numel()].copy_(plp.view(-1), non_blocking=True)
+                res.prompt_logprobs_host = host
+                self.stats["d2h_bytes"] += 4 * plp.numel()
             ev = torch.cuda.Event()
             ev.record()
             res.tokens_host, res.event = self.tokens_host, ev

@@ -379,13 +379,17 @@ class CausalLM(nn.Module):
             residual = tpc.stage_exit(residual)
         return h, residual
 
+    def lm_head(self, rows: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """This rank's vocab shard of the logits of final-normed hidden `rows` -> [R, Vp/tp] (into `out` if given)."""
+        return Fn.linear(rows, self.lm_head_w, out=out)
+
     def compute_logits(self, inp, hidden: torch.Tensor, tpc: TPComm, all_rows: bool = False,
                        local: bool = False) -> torch.Tensor:
         """Logits of the last token of every emitting sequence -> [E, V]; `local=True` returns this rank's vocab
-        shard [E, Vp/tp] instead (vocab-parallel sampling: the runner reduces winners, not logits)."""
-        hidden = tpc.materialize(hidden)
+        shard [E, Vp/tp] instead (vocab-parallel sampling: the runner reduces winners, not logits). `hidden` is the
+        final-normed activation after `tpc.materialize`."""
         rows = hidden if all_rows else Fn.gather_rows(hidden, inp.logits_idx)
-        shard = Fn.linear(rows, self.lm_head_w)
+        shard = self.lm_head(rows)
         if local:
             return shard
         return tpc.gather_logits(shard, self.spec.vocab_size)

@@ -10,7 +10,8 @@ from typing import Optional
 import torch
 
 from gllm_b200.ops import ref
-from gllm_b200.ops.ref import kv_copy_pages, logprobs_final, logprobs_shard  # noqa: F401  (sm100 signatures)
+from gllm_b200.ops.ref import (kv_copy_pages, logprobs_final, logprobs_shard,  # noqa: F401  (sm100 signatures)
+                               prompt_logprobs_shard)
 from gllm_b200.parallel import state as ps
 
 

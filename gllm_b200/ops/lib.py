@@ -76,6 +76,7 @@ def _declare(lib):
     sig("gllm_bias_rebuild", [P, L, P, I, I, I, P, P, P, P, P, P, P, P])
     sig("gllm_logprobs_shard", [P, I, L, I, I, I, P, P, P, I, P])
     sig("gllm_logprobs_final", [P, I, I, I, P, P])
+    sig("gllm_prompt_logprobs_shard", [P, I, L, I, I, I, P, P, I, P])
     sig("gllm_moe_topk_softmax", [P, L, P, P, I, I, I, I, P])
     sig("gllm_moe_grouped_topk", [P, L, P, P, P, I, I, I, I, I, I, I, F, P])
     sig("gllm_moe_align_gather", [P, P, I, I, I, P, P, I, P, P, L, P, I, P, P])

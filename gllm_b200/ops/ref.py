@@ -496,6 +496,18 @@ def logprobs_shard(logits: torch.Tensor, valid: int, n: int, tokens: torch.Tenso
     return out
 
 
+def prompt_logprobs_shard(logits: torch.Tensor, valid: int, n: int, targets: torch.Tensor, vocab_offset: int = 0,
+                          out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """PyTorch model of csrc/sample/sampler.cu:prompt_logprobs_shard_kernel (n in {0, 1}): row q of `logits` scored
+    against targets[q], in logprobs_shard's record layout — [argmax logit, its token id (lowest on ties)] when n = 1,
+    then shard max, shard sum-exp and the target's raw logit (-inf when another shard holds it)."""
+    assert n in (0, 1)
+    rec = logprobs_shard(logits, valid, n, targets, vocab_offset=vocab_offset)
+    if out is not None:
+        return out.copy_(rec)
+    return rec
+
+
 def logprobs_final(gathered: torch.Tensor, n: int) -> torch.Tensor:
     """PyTorch model of logprobs_final_kernel: [tp, E, 2n+3] records -> [E, 1 + 2n] = sampled token's log-prob, then
     n x (token id bit-cast to float, log-prob) by logit, ties to the lower id; id -1 / -inf past the vocabulary."""

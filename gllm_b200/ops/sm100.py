@@ -449,6 +449,26 @@ def logprobs_shard(logits: torch.Tensor, valid: int, n: int, tokens: torch.Tenso
     return out
 
 
+def prompt_logprobs_shard(logits: torch.Tensor, valid: int, n: int, targets: torch.Tensor, vocab_offset: int = 0,
+                          out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Prompt log-probabilities, stage 1 for n in {0, 1} (csrc/sample/sampler.cu:prompt_logprobs_shard_kernel): one
+    pass over each row of `logits` [Q, >= valid] bf16/fp32, scored against `targets` int32 [Q]; the same [Q, 2n+3]
+    record as `logprobs_shard` (written into `out` when given)."""
+    assert logits.dim() == 2 and logits.stride(1) == 1 and logits.dtype in (_BF16, torch.float32)
+    assert n in (0, 1) and targets.dtype == torch.int32 and targets.is_contiguous()
+    q = logits.shape[0]
+    assert targets.numel() == q
+    if out is None:
+        out = torch.empty(q, 2 * n + 3, dtype=torch.float32, device=logits.device)
+    assert out.shape == (q, 2 * n + 3) and out.is_contiguous() and out.dtype == torch.float32
+    L = _lib.load()
+    rc = L.gllm_prompt_logprobs_shard(_p(logits), 0 if logits.dtype == _BF16 else 1, logits.stride(0), q, valid, n,
+                                      _p(targets), _p(out), vocab_offset, stream_ptr())
+    check(rc, "prompt_logprobs_shard")
+    _count()
+    return out
+
+
 def logprobs_final(gathered: torch.Tensor, n: int) -> torch.Tensor:
     """Log-probabilities, stage 2: `gathered` [tp, E, 2n+3] (every rank's stage-1 records) -> [E, 1 + 2n] fp32: the
     sampled token's log-prob, then n x (token id bit-cast to float, log-prob), largest logit first, ties to the lower

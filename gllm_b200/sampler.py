@@ -9,6 +9,7 @@ import numpy as np
 import torch
 
 from gllm_b200.input_data import BatchArrays, InputData
+from gllm_b200.layers import functional as Fn
 from gllm_b200.parallel import state as ps
 
 
@@ -170,4 +171,30 @@ class Sampler:
         rec = self.ops.logprobs_shard(logits, valid, n, toks, rows, vocab_offset=off)
         allr = _all_gather(rec) if self.vocab_parallel else rec.unsqueeze(0)
         self.stats["logprob_rows"] = self.stats.get("logprob_rows", 0) + len(want)
+        return self.ops.logprobs_final(allr, n)
+
+    def prompt_logprobs(self, batch: BatchArrays, hidden: torch.Tensor, lm_head, tile_rows: int) -> torch.Tensor:
+        """Log-probabilities of the batch's prompt rows, each scored against its target (the next prompt token) ->
+        fp32 [Q, 1 + 2N], logprobs_final's layout. The rows' final-normed hidden states go through the LM head
+        (`lm_head(rows, out)` -> [R, Vp/tp]) `tile_rows` at a time into one reused buffer, and each tile is reduced to
+        records right after its GEMM, while it is in L2 (csrc/sample/sampler.cu: prompt_logprobs_shard_kernel, one
+        pass, for N <= 1; logprobs_shard_kernel for N > 1). The TP ranks all-gather the records of all tiles once."""
+        dev, n = hidden.device, batch.plp_n
+        rows, targets = self.inp.plp
+        q = rows.numel()
+        rec = torch.empty(q, 2 * n + 3, dtype=torch.float32, device=dev)
+        buf = None
+        for a in range(0, q, tile_rows):
+            b = min(q, a + tile_rows)
+            x = Fn.gather_rows(hidden, rows[a:b])
+            logits = lm_head(x, None if buf is None else buf[: b - a])
+            if buf is None:
+                buf = logits
+            off, valid = self._shard(logits.shape[1])
+            if n <= 1:
+                self.ops.prompt_logprobs_shard(logits, valid, n, targets[a:b], vocab_offset=off, out=rec[a:b])
+            else:
+                rec[a:b] = self.ops.logprobs_shard(logits, valid, n, targets[a:b], vocab_offset=off)
+        allr = _all_gather(rec) if ps.get_tp_size() > 1 else rec.unsqueeze(0)
+        self.stats["prompt_logprob_rows"] = self.stats.get("prompt_logprob_rows", 0) + q
         return self.ops.logprobs_final(allr, n)

@@ -64,7 +64,7 @@ PLACEHOLDER = -1  # token id of a position whose value is still being sampled on
 
 class ScheduledSeq:
     """One entry of a micro-batch: compute tokens [start, start + n) of `seq`."""
-    __slots__ = ("seq", "start", "n", "emits", "is_decode", "forks", "kv_copy")
+    __slots__ = ("seq", "start", "n", "emits", "is_decode", "forks", "kv_copy", "plp")
 
     def __init__(self, seq: Sequence, start: int, n: int):
         self.seq, self.start, self.n = seq, start, n
@@ -78,6 +78,8 @@ class ScheduledSeq:
         # the partial last prompt page. None for every other entry.
         self.forks: Optional[List[Sequence]] = None
         self.kv_copy: Optional[List[tuple]] = None
+        # prompt log-probabilities: how many prompt rows this entry carries (set when its batch is built)
+        self.plp = 0
 
     def __repr__(self):
         return f"ScheduledSeq(id={self.seq.seq_id}, start={self.start}, n={self.n})"
@@ -92,6 +94,8 @@ class SchedulerOutput:
     # aligned with next_tokens when some row of the batch asked for log-probs (entry None for rows that did not),
     # None otherwise
     next_logprobs: Optional[list] = None
+    # prompt log-probabilities delivered by the batch: seq id -> its next entries in prompt order; None when none
+    prompt_logprobs: Optional[dict] = None
 
 
 class Scheduler:
@@ -117,6 +121,7 @@ class Scheduler:
         self.batch_running: Deque[List[ScheduledSeq]] = deque()
         self.next_tokens_queue: Deque[List[int]] = deque()
         self.next_logprobs_queue: Deque[Optional[list]] = deque()   # one entry per next_tokens_queue entry
+        self.next_plp_queue: Deque[Optional[list]] = deque()        # prompt log-prob rows, likewise
         self.abort_ids = set()
         self.on_preempt = None      # callback(seq): the owner releases per-sequence device state
         self.num_preempt_seqs = 0
@@ -149,10 +154,13 @@ class Scheduler:
     def add_abort_ids(self, ids):
         self.abort_ids.update(ids)
 
-    def add_next_tokens(self, next_tokens: List[int], next_logprobs: Optional[list] = None):
-        """`next_logprobs`: None, or one entry per emitting row (None where the row did not ask)."""
+    def add_next_tokens(self, next_tokens: List[int], next_logprobs: Optional[list] = None,
+                        prompt_logprobs: Optional[list] = None):
+        """`next_logprobs`: None, or one entry per emitting row (None where the row did not ask). `prompt_logprobs`:
+        None, or one entry per prompt log-prob row of the batch, in entry order (`ScheduledSeq.plp` rows each)."""
         self.next_tokens_queue.append(next_tokens)
         self.next_logprobs_queue.append(next_logprobs)
+        self.next_plp_queue.append(prompt_logprobs)
 
     def set_log(self, log: bool):
         self.log = log
@@ -175,9 +183,21 @@ class Scheduler:
         batch = self.batch_running.popleft()
         next_tokens = self.next_tokens_queue.popleft()
         next_logprobs = self.next_logprobs_queue.popleft()
+        plp = self.next_plp_queue.popleft()
         out = SchedulerOutput()
         if next_logprobs is not None:
             out.next_logprobs = []
+        if plp is not None:
+            out.prompt_logprobs = {}
+            j = 0
+            for ent in batch:
+                if ent.plp:
+                    seq = ent.seq
+                    if not (seq.zombie or seq.is_abort):
+                        n = seq.prompt_logprobs_n       # (the batch reports its largest N for every row)
+                        out.prompt_logprobs.setdefault(seq.seq_id, []).extend(
+                            (lp, top[:n]) for lp, top in plp[j:j + ent.plp])
+                    j += ent.plp
         prefix, ps = isinstance(self.mm, PrefixMemoryManager), self.page_size
         if any(ent.forks for ent in batch):
             self._process_forks(batch, next_tokens, next_logprobs, out)
@@ -281,6 +301,9 @@ class Scheduler:
                 pairs.append((seq.page_table[full], dst))
             sib.computed_token_num = sib.scheduled_token_num = p
             sib.published = full     # the shared pages are the parent's to publish
+            # the parent's prefill scores the prompt for every choice: a fork's recompute after a preemption must not
+            # ask for those rows again
+            sib.plp_cursor = max(sib.plp_cursor, sib.prompt_len - 1)
         ent.forks, ent.kv_copy = seq.forks, (pairs or None)
         seq.forks = []
 

@@ -11,13 +11,14 @@ class Sequence:
                  "mm_contents", "page_hashes", "num_cached_tokens", "arrival_time", "first_token_time",
                  "finish_time", "slot", "mrope_delta", "mm_state", "pt_np", "pending", "zombie", "pt_gen", "published",
                  "slot_fresh", "logprobs", "output_logprobs", "seed", "frequency_penalty", "presence_penalty",
-                 "logit_bias", "forks")
+                 "logit_bias", "forks", "prompt_logprobs_n", "plp_cursor", "prompt_logprobs")
 
     def __init__(self, seq_id: int, token_ids: List[int], finish_tokens: List[int],
                  output_len: Optional[int] = None, ignore_eos: bool = False, temperature: float = 0.6,
                  top_p: float = 0.9, top_k: int = 10, repetition_penalty: float = 1.0, mm_contents=None,
                  logprobs: int = -1, seed: Optional[int] = None, frequency_penalty: float = 0.0,
-                 presence_penalty: float = 0.0, logit_bias: Optional[Dict[int, float]] = None):
+                 presence_penalty: float = 0.0, logit_bias: Optional[Dict[int, float]] = None,
+                 prompt_logprobs: int = -1):
         self.seq_id = seq_id
         self.token_ids: List[int] = list(token_ids)
         self.prompt_len = len(self.token_ids)
@@ -37,6 +38,12 @@ class Sequence:
         # (sampled token's log-prob, [(token, log-prob), ...]) per generated token, filled by the front-end
         self.logprobs = logprobs
         self.output_logprobs: list = []
+        # prompt log-probabilities (scoring): how many top alternatives to report per prompt token (-1: none); the
+        # driver's cursor, the next prompt position whose row has been requested from the model (a recompute after a
+        # preemption never asks twice); and the front-end's list, one entry per prompt token (None for the first)
+        self.prompt_logprobs_n = prompt_logprobs
+        self.plp_cursor = 0
+        self.prompt_logprobs: list = [None] if prompt_logprobs >= 0 else []
         # OpenAI sampling parameters: a seeded request draws from a stream keyed by (seed, token position), so its
         # tokens depend on its logits alone; the penalties and logit_bias form an additive row on the device
         # (`has_bias_row`), subtracted per generated occurrence / added per token id before the temperature
@@ -69,6 +76,11 @@ class Sequence:
         # and are not scheduled on their own: when its final prompt chunk is scheduled they take its full prompt
         # pages, a copy of its partial last page, and first tokens drawn from its last logits row. Emptied then.
         self.forks: List["Sequence"] = []
+
+    @property
+    def plp_pending(self) -> bool:
+        """Some prompt log-prob row has not been requested yet: the prompt's hidden states are still needed."""
+        return self.prompt_logprobs_n >= 0 and self.plp_cursor < self.prompt_len - 1
 
     @property
     def has_bias_row(self) -> bool:
