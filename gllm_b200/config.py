@@ -3,7 +3,7 @@ constructor (gllm/llm_engine.py:19-49, gllm/entrypoints/api_server.py:134-278)."
 from __future__ import annotations
 
 from dataclasses import dataclass
-from typing import List, Optional
+from typing import Dict, List, Optional
 
 
 @dataclass
@@ -45,6 +45,8 @@ class EngineConfig:
     seed: int = 0
     log_stats: bool = True
     tokenizer_path: Optional[str] = None
+    lora_modules: Optional[Dict[str, str]] = None   # multi-LoRA: adapter name -> PEFT directory (gllm_b200/lora.py)
+    max_lora_rank: int = 16                           # every adapter is zero-padded to this rank (<= 64)
 
     @property
     def world_size(self) -> int:

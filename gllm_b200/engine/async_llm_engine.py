@@ -185,7 +185,7 @@ class AsyncLLM(LLM):
     async def add_requests_async(self, raw_request, token_ids: List[int], output_len=None, ignore_eos=False,
                                  temperature=None, top_p=None, top_k=None, repetition_penalty=None,
                                  mm_contents=None, stop=None, logprobs=None, seed=None, frequency_penalty=None,
-                                 presence_penalty=None, logit_bias=None, n=None, prompt_logprobs=None):
+                                 presence_penalty=None, logit_bias=None, n=None, prompt_logprobs=None, lora=None):
         """`logprobs`: None, or N in [0, 20] — every text delta of the stream is then a `Delta` carrying the
         log-prob entries of the tokens whose text it releases (see `LLM.generate`). `seed`, `frequency_penalty`,
         `presence_penalty`, `logit_bias`: see `LLM.allocate_seq` (ValueError when out of range).
@@ -194,7 +194,7 @@ class AsyncLLM(LLM):
         `LLM.generate`; every stream's `prompt_logprobs` is the request's list, complete before its first delta."""
         seqs = self.allocate_choices(token_ids, n, output_len, ignore_eos, temperature, top_p, top_k,
                                      repetition_penalty, mm_contents, logprobs, seed, frequency_penalty,
-                                     presence_penalty, logit_bias, prompt_logprobs)
+                                     presence_penalty, logit_bias, prompt_logprobs, lora)
         streams = []
         for seq in seqs:
             stream = AsyncStream(raw_request, stop, logprobs=logprobs is not None)

@@ -159,6 +159,9 @@ class LLM:
             mm_processor_max_pixels=mm_processor_max_pixels, **extra)
         cfg = self.cfg
         self.loader = ModelLoader(cfg.model_path, cfg.load_format)
+        from gllm_b200.lora import adapter_ids
+        # multi-LoRA: adapter name -> id (0 is the base model), validated before any worker starts
+        self.lora_ids: Dict[str, int] = adapter_ids(self.loader.architecture, cfg.lora_modules, cfg.max_lora_rank)
         self.tokenizer = load_tokenizer(cfg.tokenizer_path or cfg.model_path)
         self.finish_tokens = self.loader.eos_token_ids()
         gen = self.loader.generation_config
@@ -290,13 +293,16 @@ class LLM:
 
     def allocate_seq(self, token_ids: List[int], output_len=None, ignore_eos=False, temperature=None, top_p=None,
                      top_k=None, repetition_penalty=None, mm_contents=None, logprobs=None, seed=None,
-                     frequency_penalty=None, presence_penalty=None, logit_bias=None, prompt_logprobs=None) -> Sequence:
+                     frequency_penalty=None, presence_penalty=None, logit_bias=None, prompt_logprobs=None,
+                     lora=None) -> Sequence:
         """Defaults: temperature/top_p/repetition_penalty from generation_config, top_k = 1
         (greedy) unless given (reference: gllm/llm_engine.py:305-337). `logprobs`: None (no log-probs) or the number
         N in [0, MAX_LOGPROBS] of most likely tokens to report next to every generated token's log-prob.
         `prompt_logprobs`: likewise for every prompt token after the first (`Sequence.prompt_logprobs`).
         `seed`, `frequency_penalty`, `presence_penalty`, `logit_bias`: OpenAI semantics, validated by
-        `check_sampling_params` (see entrypoints/protocol.py for the formula)."""
+        `check_sampling_params` (see entrypoints/protocol.py for the formula). `lora`: None (the base model) or the
+        name of one of the engine's `lora_modules`."""
+        lora_id = self.lora_id(lora)
         if logprobs is not None and not 0 <= int(logprobs) <= MAX_LOGPROBS:
             raise ValueError(f"logprobs must be in [0, {MAX_LOGPROBS}]")
         plp = check_prompt_logprobs(prompt_logprobs, bool(mm_contents))
@@ -315,7 +321,7 @@ class LLM:
                        1 if top_k is None else top_k,
                        self.default_repetition_penalty if repetition_penalty is None else repetition_penalty,
                        mm_contents, -1 if logprobs is None else int(logprobs), seed, frequency_penalty,
-                       presence_penalty, logit_bias, plp)
+                       presence_penalty, logit_bias, plp, lora_id)
         if output_len is None:
             seq.output_len = min(4096, self.model_max_length - len(token_ids))
         if mm_contents:
@@ -327,7 +333,7 @@ class LLM:
     def allocate_choices(self, token_ids: List[int], n=None, output_len=None, ignore_eos=False, temperature=None,
                          top_p=None, top_k=None, repetition_penalty=None, mm_contents=None, logprobs=None, seed=None,
                          frequency_penalty=None, presence_penalty=None, logit_bias=None,
-                         prompt_logprobs=None) -> List[Sequence]:
+                         prompt_logprobs=None, lora=None) -> List[Sequence]:
         """The `n` choices of one request (parallel sampling; see `check_n`): choice 0 is the request as `allocate_seq`
         makes it, choices 1..n-1 are its forks (`Sequence.forks`): the prompt is prefilled once and every choice draws
         its first token from the same logits row, then continues on its own. With a seed, choice i uses seed + i.
@@ -340,7 +346,7 @@ class LLM:
                 seqs.append(self.allocate_seq(token_ids, output_len, ignore_eos, temperature, top_p, top_k,
                                               repetition_penalty, mm_contents, logprobs,
                                               choice_seed(seed, i) if i else seed, frequency_penalty, presence_penalty,
-                                              logit_bias, prompt_logprobs))
+                                              logit_bias, prompt_logprobs, lora))
         except Exception:
             with self._inbox_lock:
                 for s in seqs:
@@ -350,6 +356,16 @@ class LLM:
         for s in seqs[1:]:
             s.prompt_logprobs = seqs[0].prompt_logprobs
         return seqs
+
+    def lora_id(self, name) -> int:
+        """Adapter id of `name` (None: 0, the base model); ValueError for a name the engine does not serve."""
+        if name is None:
+            return 0
+        if name not in self.lora_ids:
+            raise ValueError(f"unknown LoRA adapter {name!r}" + (
+                f" (this engine serves {', '.join(self.lora_ids)})" if self.lora_ids else
+                " (this engine was started without lora_modules)"))
+        return self.lora_ids[name]
 
     # The three inboxes below are filled from request handlers (event-loop thread of the API server) while the
     # engine tick runs in a worker thread: every append and the swap in `_send` hold `_inbox_lock`, so a request
@@ -448,7 +464,7 @@ class LLM:
                  repetition_penalty=None, ignore_eos: bool = False, progress: bool = False,
                  mm_contents: Optional[List[Optional[dict]]] = None, logprobs=None, seed=None,
                  frequency_penalty=None, presence_penalty=None, logit_bias=None, n=None,
-                 prompt_logprobs=None) -> List[Sequence]:
+                 prompt_logprobs=None, lora=None) -> List[Sequence]:
         """Batch generation; returns the finished `Sequence`s in request order with `.prompt`,
         `.output`, `.token_ids` (reference: gllm/llm_engine.py:343-378). `mm_contents[i]` (VL models) is
         the processor output of request i: pixel_values / image_grid_thw [/ pixel_values_videos ...].
@@ -463,7 +479,9 @@ class LLM:
         prompt token — None for the first, then (its log-prob given the tokens before it, [(token, log-prob) of the N
         most likely tokens at that position]), under the same distribution as `logprobs`; [] when not asked. Not
         available with multimodal input. Such a request takes no prefix-cache hits (it needs every prompt position's
-        hidden state); it still publishes its pages for later requests."""
+        hidden state); it still publishes its pages for later requests.
+        `lora` (multi-LoRA): None for the base model or the name of one of the engine's `lora_modules`; one value or
+        a list with one name or None per request. Requests on different adapters run in the same batches."""
         if self.worker is not None and self.worker.rank != 0:
             return self._serve_until_stop()
         if tokens is None:
@@ -481,7 +499,7 @@ class LLM:
                                             pick(repetition_penalty),
                                             mm_contents[i] if mm_contents is not None else None, pick(logprobs),
                                             pick(seed), pick(frequency_penalty), pick(presence_penalty),
-                                            pick(logit_bias), pick(prompt_logprobs))
+                                            pick(logit_bias), pick(prompt_logprobs), pick(lora))
             heads.append(choices[0])
             seqs.extend(choices)
         n = len(seqs)

@@ -35,6 +35,21 @@ def _error(msg: str, status=HTTPStatus.BAD_REQUEST):
                         status_code=status.value)
 
 
+def _route_model(request):
+    """(adapter name or None, error response or None) for the request's `model`. Without adapters every `model` is
+    served by the base model, as before; with adapters, a `model` equal to an adapter name selects it, and one that
+    names neither the base model nor an adapter is a 404 `model_not_found`."""
+    lora_ids = getattr(llm, "lora_ids", None)
+    if not lora_ids or request.model is None or request.model == str(llm.cfg.model_path):
+        return None, None
+    if request.model in lora_ids:
+        return request.model, None
+    from fastapi.responses import JSONResponse
+    return None, JSONResponse({"object": "error", "message": f"The model `{request.model}` does not exist.",
+                               "type": "NotFoundError", "param": "model", "code": "model_not_found"},
+                              status_code=HTTPStatus.NOT_FOUND.value)
+
+
 def _validate_sampling(request):
     if request.temperature is not None and request.temperature < 0:
         return "temperature must be >= 0"
@@ -351,12 +366,18 @@ def build_app(engine):
     @app.get("/v1/models")
     async def show_available_models():
         name = str(llm.cfg.model_path)
-        models = ModelList(data=[ModelCard(id=name, root=name, max_model_len=llm.model_max_length,
-                                           permission=[ModelPermission()])])
+        cards = [ModelCard(id=name, root=name, max_model_len=llm.model_max_length, permission=[ModelPermission()])]
+        for a in getattr(llm, "lora_ids", None) or ():      # one card per LoRA adapter, after the base model
+            cards.append(ModelCard(id=a, root=str(llm.cfg.lora_modules[a]), parent=name,
+                                   max_model_len=llm.model_max_length, permission=[ModelPermission()]))
+        models = ModelList(data=cards)
         return JSONResponse(content=models.model_dump())
 
     @app.post("/v1/chat/completions")
     async def create_chat_completion(request: ChatCompletionRequest, raw_request: Request):
+        lora, missing = _route_model(request)
+        if missing is not None:
+            return missing
         mm_contents = None
         try:
             if llm.loader.use_mm:
@@ -377,7 +398,7 @@ def build_app(engine):
                                               request.temperature, request.top_p, request.top_k,
                                               request.repetition_penalty, mm_contents, stop=request.stop,
                                               logprobs=(request.top_logprobs or 0) if request.logprobs else None,
-                                              **params)
+                                              lora=lora, **params)
         streams = stream if "n" in params else [stream]
         if request.stream:
             return StreamingResponse(chat_completion_stream_generator(streams, request),
@@ -386,6 +407,9 @@ def build_app(engine):
 
     @app.post("/v1/completions")
     async def create_completion(request: CompletionRequest, raw_request: Request):
+        lora, missing = _route_model(request)
+        if missing is not None:
+            return missing
         try:
             token_ids = await _in_thread(_encode_prompt, request.prompt)
         except Exception as e:  # noqa: BLE001
@@ -406,7 +430,7 @@ def build_app(engine):
         stream = await llm.add_requests_async(raw_request, token_ids, max_tokens, request.ignore_eos,
                                               request.temperature, request.top_p, request.top_k,
                                               request.repetition_penalty, stop=request.stop,
-                                              logprobs=request.logprobs, **params)
+                                              logprobs=request.logprobs, lora=lora, **params)
         streams = stream if "n" in params else [stream]
         echo = (await _in_thread(_prompt_text, request.prompt, token_ids), token_ids) if request.echo else None
         if request.stream:
@@ -474,7 +498,23 @@ def make_parser() -> argparse.ArgumentParser:
     p.add_argument("--mm-processor-min-pixels", type=int, default=None)
     p.add_argument("--mm-processor-max-pixels", type=int, default=None)
     p.add_argument("--tp-mode", type=str, default="fused", choices=["fused", "nccl"])
+    p.add_argument("--lora-modules", type=str, nargs="+", default=None, metavar="NAME=PATH",
+                   help="PEFT LoRA adapters served next to the base model; a request selects one by `model`")
+    p.add_argument("--max-lora-rank", type=int, default=16, help="every adapter is zero-padded to this rank (<= 64)")
     return p
+
+
+def parse_lora_modules(items) -> Optional[dict]:
+    """["name=path", ...] -> {name: path} (None without adapters)."""
+    if not items:
+        return None
+    out = {}
+    for it in items:
+        name, sep, path = it.partition("=")
+        if not sep or not name or not path:
+            raise ValueError(f"--lora-modules expects NAME=PATH, got {it!r}")
+        out[name] = path
+    return out
 
 
 def engine_kwargs(args) -> dict:
@@ -489,7 +529,8 @@ def engine_kwargs(args) -> dict:
                 schedule_method=args.schedule_method, disable_cuda_graph=args.disable_cuda_graph,
                 max_cuda_graph_bs=args.max_cuda_graph_bs, model_max_length=args.model_max_length,
                 mm_processor_min_pixels=args.mm_processor_min_pixels,
-                mm_processor_max_pixels=args.mm_processor_max_pixels, tp_mode=args.tp_mode)
+                mm_processor_max_pixels=args.mm_processor_max_pixels, tp_mode=args.tp_mode,
+                lora_modules=parse_lora_modules(args.lora_modules), max_lora_rank=args.max_lora_rank)
 
 
 async def run_server(app, host: str, port: int):

@@ -38,6 +38,12 @@ and `usage.completion_tokens = 0`; the engine still samples one token internally
 log-probs takes no prefix-cache hits. `prompt_logprobs` outside [0, 20] is a 400. Chat completions have no prompt
 log-probs.
 
+Multi-LoRA: a server started with `--lora-modules name=path ...` serves each PEFT adapter next to the base model. In
+chat and completions, a `model` equal to an adapter name runs the request with that adapter; the base model's id (or
+no `model`) runs the base model; any other `model` is a 404 with `code: "model_not_found"`. `/v1/models` lists the
+base model, then one card per adapter with `root` = its path and `parent` = the base model's id. Without adapters,
+`model` is not looked at and every response is what it was before.
+
 `n` asks for n independent choices of one request (parallel sampling). The prompt is prefilled once, its full KV
 pages are shared by the choices and its partial last page is copied on the device; every choice draws its first token
 from the same logits row, then continues as a sequence of its own with its own stop handling, `finish_reason` and

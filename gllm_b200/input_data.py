@@ -86,6 +86,8 @@ class BatchArrays:
     plp_rows: Optional[np.ndarray] = None    # int32 [Q]
     plp_targets: Optional[np.ndarray] = None  # int32 [Q]
     plp_n: int = -1
+    # multi-LoRA: adapter slot of every token row (-1: base model); None when no row uses an adapter
+    lora_slot: Optional[np.ndarray] = None   # int32 [T]
     emit_ids: Optional[list] = None  # driver-local: sequence id per EMITTING entry (order of the sampler output)
     seq_ids: Optional[list] = None  # driver-local: sequence id per row (incremental decode batches); not sent
     pt_gens: Optional[list] = None  # driver-local: Sequence.pt_gen per row when the block table rows were written
@@ -106,7 +108,7 @@ class BatchArrays:
                  "logits_idx", "emit_seq", "temperature", "top_k", "top_p", "rep_penalty", "state_slot"]
         opt = ["seen_rows", "seen_tokens", "clear_slots", "feed_src", "logprobs_n", "freq_pen", "pres_pen",
                "bias_slot", "rb_slots", "rb_pen", "rb_lb_off", "rb_lb_ids", "rb_lb_vals", "rb_out_off", "rb_out_toks",
-               "seed", "seed_pos", "kv_copy", "plp_rows", "plp_targets"]
+               "seed", "seed_pos", "kv_copy", "plp_rows", "plp_targets", "lora_slot"]
         scalars = (self.num_decode_seqs, self.num_seqs, self.num_tokens, self.max_q_len, self.max_seq_len,
                    self.all_greedy, self.need_penalty, self.batch_id)
         if self.need_bias:      # (only then: a batch without the feature sends the header it always sent)
@@ -209,6 +211,9 @@ def _build_decode_fast(entries, page_size: int, batch_id: int, prev: "BatchArray
         bslot = prev.bias_slot[perm]
         if (bslot >= 0).any():
             bias = dict(need_bias=True, bias_slot=bslot, freq_pen=prev.freq_pen[perm], pres_pen=prev.pres_pen[perm])
+    lora = prev.lora_slot[perm] if prev.lora_slot is not None else None
+    if lora is not None and not (lora >= 0).any():
+        lora = None        # the adapter rows have finished
     seed = seed_pos = None
     if prev.seed_pos is not None:
         seed_pos = prev.seed_pos[perm]
@@ -223,7 +228,7 @@ def _build_decode_fast(entries, page_size: int, batch_id: int, prev: "BatchArray
         rep_penalty=prev.rep_penalty[perm], state_slot=prev.state_slot[perm],
         logprobs_n=lp_n, num_decode_seqs=b, num_seqs=b, num_tokens=b, max_q_len=1,
         max_seq_len=int(seq_lens.max()), all_greedy=prev.all_greedy, need_penalty=False, batch_id=batch_id,
-        seq_ids=ids, emit_ids=ids, pt_gens=gens, seed=seed, seed_pos=seed_pos, **bias)
+        seq_ids=ids, emit_ids=ids, pt_gens=gens, seed=seed, seed_pos=seed_pos, lora_slot=lora, **bias)
 
 
 def _bias_fields(freq_pen, pres_pen, bias_slot, rb_slots, rb_pen, rb_lb_off, rb_lb_ids, rb_lb_vals, rb_out_off,
@@ -373,6 +378,9 @@ def build_batch(entries, page_size: int, vocab_size: int, batch_id: int = 0, mro
                 n = entries[i].n
                 seen_rows.append(np.full(n, seq.slot, dtype=np.int32))
                 seen_tokens.append(np.asarray(seq.token_ids[end - n:end], dtype=np.int32))
+    lora_slot = None
+    if any(e.seq.lora_id for e in entries):
+        lora_slot = np.repeat(np.fromiter((e.seq.lora_id - 1 for e in entries), dtype=np.int32, count=b), q_lens)
     mm = None
     if mrope:
         from gllm_b200.models.multimodal import batch_mm_payload
@@ -393,7 +401,7 @@ def build_batch(entries, page_size: int, vocab_size: int, batch_id: int = 0, mro
         seed_pos=np.asarray(seed_pos, dtype=np.int32) if want_seed else None,
         kv_copy=np.asarray(kv_copy, dtype=np.int32).reshape(-1, 2) if kv_copy else None,
         plp_rows=np.concatenate(plp_rows) if plp_rows else None,
-        plp_targets=np.concatenate(plp_targets) if plp_rows else None, plp_n=plp_n,
+        plp_targets=np.concatenate(plp_targets) if plp_rows else None, plp_n=plp_n, lora_slot=lora_slot,
         **(_bias_fields(freq_pen, pres_pen, bias_slot, rb_slots, rb_pen, rb_lb_off, rb_lb_ids, rb_lb_vals, rb_out_off,
                         rb_out_toks) if need_bias else {}),
         seq_ids=[e.seq.seq_id for e in entries] if n_dec == b else None,
@@ -444,12 +452,41 @@ class InputData:
         self._seed_pos = buf((max_seqs,), i32)
         self._buf = buf
         self._plp = None   # (rows, targets) of prompt log-prob rows: allocated by the first batch that has them
+        self.lora_adapters = 0   # number of adapters the engine serves (`set_lora`)
+        self.lora_groups = 0     # adapter groups of the loaded batch (the graph capture pins it to lora_adapters)
+        self._lora_h2d = 0
         self.need_tok_seq = False  # MLA attention wants token -> sequence for mixed / prefill batches
         self.batch: Optional[BatchArrays] = None
         self.num_tokens = self.num_seqs = self.num_decode_seqs = self.num_emit = 0
         self.max_q_len = self.max_seq_len = 0
         self.padded_tokens = 0  # > 0 when padded to a CUDA-graph bucket
         self.decode_splits = None  # None: pick per batch (eager); int: fixed (CUDA graphs)
+
+    def set_lora(self, num_adapters: int):
+        """Allocate the per-batch adapter CSR (see csrc/lora/lora.cu): slots [L], row_off [L + 1], rows [T]."""
+        self.lora_adapters = num_adapters
+        self._lora = (self._buf((num_adapters,), torch.int32), self._buf((num_adapters + 1,), torch.int32),
+                      self._buf((self.max_tokens,), torch.int32))
+
+    def _load_lora(self, lora_slot: np.ndarray):
+        """Group the token rows by adapter: the S active slots in increasing order, then the rows without one. row_off
+        is padded to L + 1 entries with the end of the adapter rows, so a kernel launched for L groups (CUDA graphs)
+        sees the extra groups empty."""
+        n_ad = self.lora_adapters
+        key = np.where(lora_slot < 0, n_ad, lora_slot)
+        rows = np.argsort(key, kind="stable").astype(np.int32)
+        counts = np.bincount(key, minlength=n_ad + 1)[:n_ad]
+        slots = np.nonzero(counts)[0].astype(np.int32)
+        off = np.empty(n_ad + 1, dtype=np.int32)
+        off[0] = 0
+        np.cumsum(counts[slots], out=off[1:slots.shape[0] + 1])
+        off[slots.shape[0] + 1:] = off[slots.shape[0]]
+        self.lora_groups = int(slots.shape[0])
+        if slots.shape[0]:
+            self._put(self._lora[0], slots)
+        self._put(self._lora[1], off)
+        self._put(self._lora[2], rows)
+        self._lora_h2d = slots.nbytes + off.nbytes + rows.nbytes
 
     def _put(self, pair, arr: np.ndarray):
         """numpy array -> this step's pinned staging buffer (plain numpy store through a shared-memory view: no
@@ -493,6 +530,8 @@ class InputData:
                 self._plp = (self._buf((self.max_tokens,), torch.int32), self._buf((self.max_tokens,), torch.int32))
             self._put(self._plp[0], batch.plp_rows)
             self._put(self._plp[1], batch.plp_targets)
+        if batch.lora_slot is not None:
+            self._load_lora(batch.lora_slot)
         self._put(self._block_table, batch.block_table)
         self._put(self._seq_lens, batch.seq_lens)
         self._put(self._qsl, batch.query_start_loc)
@@ -539,6 +578,8 @@ class InputData:
         self._block_table[1][b:bucket, 0].fill_(dummy_page)
         self._seq_lens[1][b:bucket].fill_(1)
         self._qsl[1][b:bucket + 1].copy_(torch.arange(b, bucket + 1, dtype=torch.int32, device=self.device))
+        if self.batch.lora_slot is not None:     # padding rows: no adapter (the last CSR group runs them as base rows)
+            self._lora[2][1][b:bucket].copy_(torch.arange(b, bucket, dtype=torch.int32, device=self.device))
         self.padded_tokens = bucket
 
     # -- views ------------------------------------------------------------------------------------
@@ -604,6 +645,14 @@ class InputData:
         return self._bias_slot[1][: self.num_emit] if self.batch is not None and self.batch.need_bias else None
 
     @property
+    def lora(self):
+        """(slots, row_off, rows, number of groups) of the batch's adapter CSR, or None when no row uses an adapter."""
+        if self.batch is None or self.batch.lora_slot is None:
+            return None
+        l1 = self._lora
+        return l1[0][1], l1[1][1], l1[2][1][: self._n_tok()], self.lora_groups
+
+    @property
     def plp(self):
         """(int32 rows [Q], int32 targets [Q]) of the batch's prompt log-prob rows on the device."""
         q = self.batch.plp_rows.shape[0]
@@ -627,4 +676,6 @@ class InputData:
         for a in (b.freq_pen, b.pres_pen, b.bias_slot, b.seed, b.seed_pos, b.plp_rows, b.plp_targets):
             if a is not None:
                 tot += a.nbytes
+        if b.lora_slot is not None:
+            tot += self._lora_h2d
         return tot

@@ -80,3 +80,22 @@ def paged_attention(q, k_cache, v_cache, inp, scale, num_q_heads, head_dim):
     return ref.paged_attention(q, k_cache, v_cache, inp.block_table, inp.seq_lens, inp.query_start_loc, scale,
                                num_q_heads, head_dim)
 
+
+
+def lora_shrink(x, A, csr):
+    """`csr` = (slots, row_off, rows, number of groups) of the batch (InputData.lora)."""
+    if x.is_cuda:
+        return _sm().lora_shrink(x, A, *csr)
+    return ref.lora_shrink(x, A, *csr[:3])
+
+
+def lora_expand_add(y, u, B, bounds, csr):
+    if y.is_cuda:
+        return _sm().lora_expand_add(y, u, B, bounds, *csr)
+    return ref.lora_expand_add(y, u, B, bounds, *csr[:3])
+
+
+def lora_expand_silu_mul(pre, u, B, csr):
+    if pre.is_cuda:
+        return _sm().lora_expand_silu_mul(pre, u, B, *csr)
+    return ref.lora_expand_silu_mul(pre, u, B, *csr[:3])

@@ -128,7 +128,12 @@ class PrefixMemoryManager(MemoryManager):
         while len(hs) < upto_pages:
             i = len(hs)
             # multimodal prompts share placeholder ids: salt the chain with a digest of the pixels
-            prev = hs[-1] if hs else 0x9E3779B97F4A7C15 ^ ((seq.mm_state or {}).get("salt", 0))
+            if hs:
+                prev = hs[-1]
+            else:
+                prev = 0x9E3779B97F4A7C15 ^ ((seq.mm_state or {}).get("salt", 0))
+                if seq.lora_id:    # an adapter's KV differs from the base model's and every other adapter's
+                    prev = hash((prev, -1, seq.lora_id))
             hs.append(hash((prev, tuple(toks[i * ps:(i + 1) * ps]))))
 
     # -- allocation -----------------------------------------------------------------------------

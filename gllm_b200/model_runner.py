@@ -111,12 +111,13 @@ class ModelRunner:
         self.input_data: Optional[InputData] = None
         self.tpc = None
         self.graphs: Dict[int, object] = {}
+        self.lora = None                           # lora.LoraStore when the engine serves adapters
+        self.lora_graphs: Dict[int, object] = {}   # decode buckets captured with the adapter kernels
         self.num_pages = 0
         self.device = None
         self.sampler: Optional[Sampler] = None
         self.stats = {"steps": 0, "graph_steps": 0, "tokens": 0, "h2d_bytes": 0, "d2h_bytes": 0,
                       "graph_kernel_launches": 0, "gpu_ms": 0.0}
-        self.graph_kernels: Dict[int, int] = {}
         self.time_steps = False   # bench: bracket every step with CUDA events
         self._step_events = []
 
@@ -141,7 +142,8 @@ class ModelRunner:
         self.spec = self.model.spec
         want_fused = cfg.tp_mode == "fused" and cfg.tp_size > 1 and is_cuda
         why_not = "fp8 block-scaled linears" if getattr(self.spec, "quant", None) is not None else \
-            "DeepStack (Qwen3-VL) feature injection" if getattr(self.model, "num_deepstack", 0) else None
+            "DeepStack (Qwen3-VL) feature injection" if getattr(self.model, "num_deepstack", 0) else \
+            "LoRA adapters" if cfg.lora_modules else None
         if want_fused and why_not:
             logger.warning("tp_mode=fused is not available with %s: tensor-parallel collectives run on NCCL", why_not)
         self.tpc = make_tp_comm(fused=(want_fused and why_not is None),
@@ -153,6 +155,13 @@ class ModelRunner:
         self.input_data = InputData(self.max_num_batched_tokens, max(self.max_running_seqs, 1), max_blocks,
                                     self.device, mrope=mrope)
         self.input_data.need_tok_seq = bool(self.loader.use_mla)
+        if cfg.lora_modules:
+            # before the profile run, so that the KV-cache sizing sees the adapter weights
+            from gllm_b200.lora import LoraStore
+            self.lora = LoraStore(cfg.lora_modules, cfg.max_lora_rank, self.model, self.device)
+            self.input_data.set_lora(self.lora.num_adapters)
+            logger.info("LoRA: %d adapters at rank %d, %.1f MB on this rank", self.lora.num_adapters,
+                        self.lora.rank, self.lora.nbytes / 2 ** 20)
         # test hook (tests/mp_tp_check.py): keep the full last-token logits of every step, per emitting sequence id
         self.keep_logits = os.environ.get("GLLM_KEEP_LOGITS", "0") == "1"
         self.logit_log = []
@@ -196,7 +205,7 @@ class ModelRunner:
             return
         t = self.max_num_batched_tokens
         n = max(1, min(self.max_running_seqs, t))
-        batch = _dummy_batch(t, n, self.page_size, self.input_data.max_blocks)
+        batch = _dummy_batch(t, n, self.page_size, self.input_data.max_blocks, lora=self.lora is not None)
         torch.cuda.synchronize()
         hidden = residual = None
         if not ps.is_first_pp_rank():     # later stages start from the previous stage's (hidden, residual)
@@ -261,20 +270,33 @@ class ModelRunner:
         return max(1, min(self.PLP_TILE_ROWS, self.max_running_seqs))
 
     def capture_graphs(self):
-        """Decode-only batches replay a CUDA graph per power-of-two bucket (forward -> logits)."""
-        inp = self.input_data
+        """Decode-only batches replay a CUDA graph per power-of-two bucket (forward -> logits). An engine with
+        adapters captures a second set with the LoRA kernels, replayed by decode batches that have adapter rows."""
         self.graph_pool = None
-        self.graph_logits: Dict[int, torch.Tensor] = {}
-        self.graph_hidden: Dict[int, tuple] = {}
         from gllm_b200.ops import sm100
-        kvh, _ = self.kv_shape()
         sm100.reserve_attn_workspace(self.device, max(self.capture_sizes or [1]), self.model.layers[0].attn.num_heads
                                      if len(self.model.layers) else 1, self.model.head_dim)
-        dummy_page = self.num_pages - 1
         t0 = time.time()
+        self._capture_set(self.graphs, lora=False)
+        logger.info("captured %d CUDA graphs (buckets %s) in %.1fs", len(self.graphs), self.capture_sizes,
+                    time.time() - t0)
+        if self.lora is not None:
+            t0 = time.time()
+            free0 = torch.cuda.mem_get_info(self.device)[0]
+            self._capture_set(self.lora_graphs, lora=True)
+            logger.info("captured %d LoRA CUDA graphs in %.1fs, %.1f MB of graph memory", len(self.lora_graphs),
+                        time.time() - t0, (free0 - torch.cuda.mem_get_info(self.device)[0]) / 2 ** 20)
+
+    def _capture_set(self, graphs: Dict[int, object], lora: bool):
+        inp = self.input_data
+        from gllm_b200.ops import sm100
+        kvh, _ = self.kv_shape()
+        dummy_page = self.num_pages - 1
         for bs in self.capture_sizes:
-            batch = _dummy_batch(bs, bs, self.page_size, inp.max_blocks, page=dummy_page, decode=True)
+            batch = _dummy_batch(bs, bs, self.page_size, inp.max_blocks, page=dummy_page, decode=True, lora=lora)
             inp.load(batch)
+            if lora:
+                inp.lora_groups = self.lora.num_adapters   # every adapter's group: a replay finds the others empty
             inp.padded_tokens = bs
             inp.decode_splits = sm100.decode_splits(bs, max(kvh, 1), self.model.layers[0].attn.num_heads
                                                     if len(self.model.layers) else 1, self.model_max_length)
@@ -292,20 +314,15 @@ class ModelRunner:
             n0 = sm100.launches()
             with torch.cuda.graph(g, pool=self.graph_pool):
                 out, r = self._forward_loaded(hid, res, all_rows=True)
-            self.graph_kernels[bs] = sm100.launches() - n0
             self.graph_pool = self.graph_pool or g.pool()
-            self.graphs[bs] = (g, inp.decode_splits)
-            if ps.is_last_pp_rank():
-                self.graph_logits[bs] = out
-            else:
-                self.graph_hidden[bs] = (out, r)
+            # (g, decode splits, kernel launches, logits | (hidden, residual))
+            graphs[bs] = (g, inp.decode_splits, sm100.launches() - n0,
+                          out if ps.is_last_pp_rank() else (out, r))
         inp.decode_splits = None
         inp.padded_tokens = 0
         torch.cuda.synchronize()
         if ps.get_world_size() > 1 and torch.distributed.is_initialized():
             torch.distributed.barrier()
-        logger.info("captured %d CUDA graphs (buckets %s) in %.1fs", len(self.graphs), self.capture_sizes,
-                    time.time() - t0)
 
     # -------------------------------------------------------------------------------------------
     def step(self, batch: BatchArrays, hidden: Optional[torch.Tensor] = None,
@@ -371,16 +388,19 @@ class ModelRunner:
             recv_tiles = None
         if bucket is not None:
             assert batch.plp_rows is None, "a decode-only batch carries no prompt rows"
-            g, splits = self.graphs[bucket]
+            if batch.lora_slot is not None:
+                g, splits, launches, out = self.lora_graphs[bucket]
+                self.stats["lora_graph_steps"] = self.stats.get("lora_graph_steps", 0) + 1
+            else:
+                g, splits, launches, out = self.graphs[bucket]
             inp.pad_for_graph(bucket, (self.num_pages - 1) * self.page_size, self.num_pages - 1)
             g.replay()
             self.stats["graph_steps"] += 1
-            self.stats["graph_kernel_launches"] += self.graph_kernels.get(bucket, 0)
+            self.stats["graph_kernel_launches"] += launches
             inp.padded_tokens = 0
             if ps.is_last_pp_rank():
-                logits = self.graph_logits[bucket][: batch.num_seqs]
-                return self._sample(batch, logits)
-            h, r = self.graph_hidden[bucket]
+                return self._sample(batch, out[: batch.num_seqs])
+            h, r = out
             return StepResult(hidden=h[: batch.num_tokens], residual=r[: batch.num_tokens])
         out, r = self._forward_loaded(hidden, residual, recv_tiles=recv_tiles)
         if ps.is_last_pp_rank():
@@ -444,15 +464,16 @@ class ModelRunner:
         if self.device is not None and torch.device(self.device).type == "cuda":
             torch.cuda.synchronize()
         self.graphs.clear()
+        self.lora_graphs.clear()
         tpc, self.tpc = self.tpc, None
         if tpc is not None and hasattr(tpc, "close"):
             tpc.close()
 
 
 def _dummy_batch(num_tokens: int, num_seqs: int, page_size: int, max_blocks: int, page: int = 0,
-                 decode: bool = False) -> BatchArrays:
+                 decode: bool = False, lora: bool = False) -> BatchArrays:
     """Synthetic batch for the memory probe / graph capture: `num_seqs` sequences sharing the
-    tokens evenly (decode=True: one token each, KV length 1 on `page`)."""
+    tokens evenly (decode=True: one token each, KV length 1 on `page`); `lora`: every row on adapter slot 0."""
     if decode:
         q = np.ones(num_seqs, dtype=np.int32)
     else:
@@ -471,4 +492,5 @@ def _dummy_batch(num_tokens: int, num_seqs: int, page_size: int, max_blocks: int
         emit_seq=np.arange(e, dtype=np.int32), temperature=np.ones(e, np.float32), top_k=np.ones(e, np.int32),
         top_p=np.ones(e, np.float32), rep_penalty=np.ones(e, np.float32), state_slot=np.zeros(e, np.int32),
         num_decode_seqs=num_seqs if decode else 0, num_seqs=num_seqs, num_tokens=t, max_q_len=int(q.max()),
-        max_seq_len=int(q.max()), all_greedy=True, need_penalty=False)
+        max_seq_len=int(q.max()), all_greedy=True, need_penalty=False,
+        lora_slot=np.zeros(t, np.int32) if lora else None)

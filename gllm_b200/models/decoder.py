@@ -167,11 +167,15 @@ class Attention(nn.Module):
     def qkv_proj(self, h: torch.Tensor, tpc: TPComm) -> torch.Tensor:
         return tpc.col_linear(h, _qw(self.qkv_w, self.qkv_ws), self.qkv_b)
 
-    def forward(self, inp, h: torch.Tensor, kv_cache, tpc: TPComm, qkv: Optional[torch.Tensor] = None) -> torch.Tensor:
+    def forward(self, inp, h: torch.Tensor, kv_cache, tpc: TPComm, qkv: Optional[torch.Tensor] = None,
+                lora=None) -> torch.Tensor:
         """h [T, H] (normed) -> attention output [T, q_size] (input of the row-parallel O-proj).
-        `qkv` may be supplied pre-computed (tile-streamed pipeline input)."""
+        `qkv` may be supplied pre-computed (tile-streamed pipeline input). `lora`: the layer's adapters when the
+        batch has adapter rows (their deltas go into q/k/v before RoPE and the KV write)."""
         if qkv is None:
             qkv = self.qkv_proj(h, tpc)
+        if lora is not None:
+            lora.add("qkv", inp.lora, h, qkv)
         t = qkv.shape[0]
         d = self.head_dim
         q = qkv[:, : self.q_size].view(t, self.num_heads, d)
@@ -213,7 +217,14 @@ class DenseMLP(nn.Module):
     def down_weight(self):
         return _qw(self.down_w, self.down_ws)
 
-    def act(self, h: torch.Tensor, tpc: TPComm) -> torch.Tensor:
+    def act(self, h: torch.Tensor, tpc: TPComm, lora=None, csr=None) -> torch.Tensor:
+        if lora is not None:
+            # adapter rows: the plain GEMM's pre-activations, then the deltas and the activation in one pass
+            if self.fused_act:
+                return lora.silu_mul(csr, h, tpc.col_linear(h, self.gate_up_w))
+            pre = tpc.col_linear(h, _qw(self.gate_up_w, self.gate_up_ws))
+            lora.add("gate_up", csr, h, pre)
+            return Fn.silu_and_mul(pre)
         if self.fused_act:
             return tpc.col_linear_silu_mul(h, self.gate_up_w)
         return Fn.silu_and_mul(tpc.col_linear(h, _qw(self.gate_up_w, self.gate_up_ws)))
@@ -234,6 +245,7 @@ class DecoderLayer(nn.Module):
             self.mlp = moe_factory(spec, layer_id, device)
         else:
             self.mlp = DenseMLP(h, spec.intermediate_size, dt, device, spec=spec)
+        self.lora = None   # lora.LoraLayer when the engine serves adapters
 
     def forward(self, inp, h: torch.Tensor, residual: torch.Tensor, kv_cache, tpc: TPComm,
                 next_norm_w: Optional[torch.Tensor], qkv: Optional[torch.Tensor] = None):
@@ -241,16 +253,23 @@ class DecoderLayer(nn.Module):
         Returns (normed input of the next block, residual) — or (un-normed block output, residual)
         when `next_norm_w` is None (last layer of a non-final pipeline stage)."""
         eps = self.spec.rms_eps
-        a = self.attn(inp, h, kv_cache, tpc, qkv=qkv)
-        h, residual = tpc.row_linear_add_norm(a, _qw(self.attn.o_w, self.attn.o_ws), residual, self.post_norm_w, eps, self.attn.o_b)
+        # adapters only when the batch has adapter rows: a base-only batch runs exactly the plain forward
+        lo = self.lora if self.lora is not None and inp is not None and inp.lora is not None else None
+        csr = inp.lora if lo is not None else None
+        a = self.attn(inp, h, kv_cache, tpc, qkv=qkv, lora=lo)
+        # row-parallel o / down: each rank adds its partial delta (its K-slice of A) before the sum over ranks
+        delta = (lambda y: lo.add("o", csr, a, y)) if lo is not None else None
+        h, residual = tpc.row_linear_add_norm(a, _qw(self.attn.o_w, self.attn.o_ws), residual, self.post_norm_w, eps,
+                                              self.attn.o_b, delta=delta)
         if self.is_moe:
             if next_norm_w is None:
                 return tpc.all_reduce(self.mlp(tpc.materialize(h), tpc)), residual
             return tpc.moe_add_norm(self.mlp, h, residual, next_norm_w, eps)
-        act = self.mlp.act(h, tpc)
+        act = self.mlp.act(h, tpc, lo, csr)
+        delta = (lambda y: lo.add("down", csr, act, y)) if lo is not None else None
         if next_norm_w is None:
-            return tpc.row_linear(act, self.mlp.down_weight()), residual
-        return tpc.row_linear_add_norm(act, self.mlp.down_weight(), residual, next_norm_w, eps)
+            return tpc.row_linear(act, self.mlp.down_weight(), delta=delta), residual
+        return tpc.row_linear_add_norm(act, self.mlp.down_weight(), residual, next_norm_w, eps, delta=delta)
 
 
 class CausalLM(nn.Module):

@@ -85,6 +85,9 @@ def _declare(lib):
     sig("gllm_fp8_quant_group", [P, L, P, P, I, I, P])
     sig("gllm_moe_grouped_gemm_fp8", [P, P, P, P, P, L, I, I, I, I, P, P, I, P])
     sig("gllm_gemm_fp8_block", [P, P, P, P, P, L, I, I, I, P, P])
+    sig("gllm_lora_shrink", [P, L, P, P, P, I, I, I, P, P, P, I, I, P])
+    sig("gllm_lora_expand_add", [P, L, P, P, L, I, I, I, I, I, I, P, P, P, I, P])
+    sig("gllm_lora_expand_silu_mul", [P, L, P, L, P, P, L, I, I, I, P, P, P, I, P])
 
 
 def load():

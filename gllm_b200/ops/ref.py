@@ -627,3 +627,53 @@ def merge_attn_states(o1: torch.Tensor, lse1: torch.Tensor, o2: torch.Tensor, ls
     den = w1 + w2
     o = (o1.float() * (w1 / den).unsqueeze(-1) + o2.float() * (w2 / den).unsqueeze(-1)).to(o1.dtype)
     return o, m + torch.log(den)
+
+
+# ----------------------------------------------------------------------------------------------
+# multi-LoRA (csrc/lora/lora.cu). Rows are grouped per adapter by the batch CSR: slots [S], row_off [S + 1] and
+# rows [T] (the adapter groups first, then the rows without an adapter).
+# ----------------------------------------------------------------------------------------------
+def _lora_groups(slots, row_off, rows):
+    off = row_off.tolist()
+    for g, s in enumerate(slots.tolist()):
+        if off[g + 1] > off[g]:
+            yield s, rows[off[g]:off[g + 1]].long()
+
+
+def lora_shrink(x: torch.Tensor, A: torch.Tensor, slots, row_off, rows) -> torch.Tensor:
+    """U [T, M] fp32 = x [T, K] · A[slot(row)] [M, K]ᵀ for every row of an adapter group, 0 for the others."""
+    u = torch.zeros(x.shape[0], A.shape[1], dtype=torch.float32, device=x.device)
+    for s, r in _lora_groups(slots, row_off, rows):
+        u[r] = x[r].float() @ A[s].float().t()
+    return u
+
+
+def lora_delta(u: torch.Tensor, B: torch.Tensor, bounds, slots, row_off, rows) -> torch.Tensor:
+    """fp32 [T, N] delta: column n of module m (bounds[m] <= n < bounds[m + 1]) is U[:, m·r : (m+1)·r] · B[slot, n]."""
+    r = B.shape[2]
+    d = torch.zeros(u.shape[0], B.shape[1], dtype=torch.float32, device=u.device)
+    for s, rr in _lora_groups(slots, row_off, rows):
+        for m in range(len(bounds) - 1):
+            a, b = bounds[m], bounds[m + 1]
+            d[rr, a:b] = u[rr, m * r:(m + 1) * r] @ B[s, a:b].float().t()
+    return d
+
+
+def lora_expand_add(y: torch.Tensor, u: torch.Tensor, B: torch.Tensor, bounds, slots, row_off, rows) -> torch.Tensor:
+    """y [T, N] += delta (fp32 sum, one rounding to y's dtype), in place."""
+    y.copy_((y.float() + lora_delta(u, B, bounds, slots, row_off, rows)).to(y.dtype))
+    return y
+
+
+def lora_expand_silu_mul(pre: torch.Tensor, u: torch.Tensor, B: torch.Tensor, slots, row_off, rows,
+                         block: int = 128) -> torch.Tensor:
+    """pre [T, 2I] gate/up pre-activations interleaved per `block` rows (see interleave_gate_up), u [T, 2r] (gate's
+    shrink then up's), B [L, 2I, r] interleaved like the weight -> SiLU(gate + dg) · (up + du) [T, I]."""
+    t, two_i = pre.shape
+    r = B.shape[2]
+    gate_col = (torch.arange(two_i, device=pre.device) % (2 * block)) < block
+    d = torch.zeros(t, two_i, dtype=torch.float32, device=pre.device)
+    for s, rr in _lora_groups(slots, row_off, rows):
+        d[rr] = torch.where(gate_col, u[rr, :r] @ B[s].float().t(), u[rr, r:2 * r] @ B[s].float().t())
+    y = (pre.float() + d).reshape(t, two_i // (2 * block), 2, block)
+    return (F.silu(y[:, :, 0]) * y[:, :, 1]).to(pre.dtype).reshape(t, two_i // 2)

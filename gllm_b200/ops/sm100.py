@@ -655,3 +655,60 @@ def mla_attention(q_full: torch.Tensor, cache: torch.Tensor, block_table: torch.
                                stream_ptr()), "mla_attention")
     _count(2 if splits > 1 else 1)
     return out
+
+
+# ----------------------------------------------------------------------------------------------
+# multi-LoRA (csrc/lora/lora.cu); slots / row_off / rows: the batch CSR (see ops.ref.lora_shrink)
+# ----------------------------------------------------------------------------------------------
+def lora_k_splits(t: int, k: int, m: int) -> int:
+    """K-slices per shrink tile: enough CTAs to spread A over the SMs when few row tiles exist (decode)."""
+    tiles = ((m + 63) // 64) * ((t + 63) // 64)
+    return max(1, min(k // 128, (2 * NUM_SMS + tiles - 1) // tiles))
+
+
+def lora_shrink(x: torch.Tensor, A: torch.Tensor, slots: torch.Tensor, row_off: torch.Tensor, rows: torch.Tensor,
+                num_groups: int) -> torch.Tensor:
+    """U [T, M] fp32 = x [T, K] · A[slot] [M, K]ᵀ per adapter group; 0 for rows without an adapter. `rows` lists every
+    one of the T rows. Deterministic: K-sliced partial sums are added in a fixed order."""
+    assert x.dtype == _BF16 and A.dtype == _BF16 and A.is_contiguous() and x.stride(1) == 1
+    t, k = x.shape
+    m = A.shape[1]
+    assert rows.shape[0] == t, (rows.shape, t)
+    u = torch.empty(t, m, dtype=torch.float32, device=x.device)
+    splits = lora_k_splits(t, k, m)
+    ws = torch.empty(splits * t * m, dtype=torch.float32, device=x.device) if splits > 1 else None
+    L = _lib.load()
+    check(L.gllm_lora_shrink(_p(x), x.stride(0), _p(A), _p(u), _p(ws), t, k, m, _p(slots), _p(row_off), _p(rows),
+                             num_groups, splits, stream_ptr()), "lora_shrink")
+    _count(2 if splits > 1 and num_groups > 0 else 1)
+    return u
+
+
+def lora_expand_add(y: torch.Tensor, u: torch.Tensor, B: torch.Tensor, bounds, slots: torch.Tensor,
+                    row_off: torch.Tensor, rows: torch.Tensor, num_groups: int) -> torch.Tensor:
+    """y [T, N] += U_m · B_m[slot]ᵀ in place; `bounds` = column offsets of the (up to three) modules, ending at N."""
+    assert y.dtype == _BF16 and y.stride(1) == 1 and B.dtype == _BF16 and B.is_contiguous()
+    assert u.dtype == torch.float32 and u.stride(1) == 1 and len(bounds) in (2, 3, 4) and bounds[-1] == y.shape[1]
+    n, r = B.shape[1], B.shape[2]
+    nb = list(bounds[1:-1]) + [n, n]
+    L = _lib.load()
+    check(L.gllm_lora_expand_add(_p(u), u.stride(0), _p(B), _p(y), y.stride(0), y.shape[0], n, r, nb[0], nb[1],
+                                 (len(bounds) - 1) * r, _p(slots), _p(row_off), _p(rows), num_groups, stream_ptr()),
+          "lora_expand_add")
+    _count()
+    return y
+
+
+def lora_expand_silu_mul(pre: torch.Tensor, u: torch.Tensor, B: torch.Tensor, slots: torch.Tensor,
+                         row_off: torch.Tensor, rows: torch.Tensor, num_groups: int) -> torch.Tensor:
+    """SiLU(gate + dg) · (up + du) [T, I] from the 128-interleaved gate/up pre-activations pre [T, 2I]."""
+    assert pre.dtype == _BF16 and pre.stride(1) == 1 and B.dtype == _BF16 and B.is_contiguous()
+    t, two_i = pre.shape
+    r = B.shape[2]
+    out = torch.empty(t, two_i // 2, dtype=_BF16, device=pre.device)
+    L = _lib.load()
+    check(L.gllm_lora_expand_silu_mul(_p(pre), pre.stride(0), _p(u), u.stride(0), _p(B), _p(out), out.stride(0), t,
+                                      two_i // 2, r, _p(slots), _p(row_off), _p(rows), num_groups, stream_ptr()),
+          "lora_expand_silu_mul")
+    _count()
+    return out

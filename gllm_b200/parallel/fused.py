@@ -316,7 +316,8 @@ class FusedTPComm(TPComm):
             return sm100.linear_silu_mul(x, w_interleaved)
         return sm100.linear_silu_mul(x, w_interleaved, comm=comm)
 
-    def row_linear_add_norm(self, x, w, residual, norm_w, eps, bias=None):
+    def row_linear_add_norm(self, x, w, residual, norm_w, eps, bias=None, delta=None):
+        assert delta is None, "LoRA deltas run on the NCCL strategy (the partial output is never materialised here)"
         from gllm_b200.ops import sm100
         if self.small:
             # decode-sized T: best local GEMM for the shape (swap-AB / split-K), then the one-kernel
@@ -510,7 +511,8 @@ class FusedTPComm(TPComm):
         shifted = _ShiftedRows(out, r0)
         return self._reduce_norm(0, 0, shifted, residual is not None, norm_w, eps)
 
-    def row_linear(self, x, w, bias=None):
+    def row_linear(self, x, w, bias=None, delta=None):
+        assert delta is None, "LoRA deltas run on the NCCL strategy"
         if self.small:
             return super().row_linear(x, w, bias)
         raise NotImplementedError("fused TP is used with pp_size == 1 (no un-normalised stage boundary)")

@@ -15,7 +15,7 @@ patterns of a block:
 """
 from __future__ import annotations
 
-from typing import Optional
+from typing import Callable, Optional
 
 import torch
 
@@ -75,13 +75,20 @@ class TPComm:
         return self.reduce_add_norm(partial, residual, norm_w, eps)
 
     def row_linear_add_norm(self, x: torch.Tensor, w: torch.Tensor, residual: Optional[torch.Tensor],
-                            norm_w: torch.Tensor, eps: float, bias: Optional[torch.Tensor] = None):
+                            norm_w: torch.Tensor, eps: float, bias: Optional[torch.Tensor] = None,
+                            delta: Optional[Callable[[torch.Tensor], None]] = None):
+        """`delta(partial)` (LoRA) adds to this rank's partial GEMM output in place, before the sum over ranks."""
         # bias is added once (rank 0) like the reference (gllm/layers/linear.py:230-258)
         partial = Fn.linear(x, w, bias if self.tp_rank == 0 else None)
+        if delta is not None:
+            delta(partial)
         return self.reduce_add_norm(partial, residual, norm_w, eps)
 
-    def row_linear(self, x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None) -> torch.Tensor:
+    def row_linear(self, x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None,
+                   delta: Optional[Callable[[torch.Tensor], None]] = None) -> torch.Tensor:
         out = Fn.linear(x, w, bias if self.tp_rank == 0 else None)
+        if delta is not None:
+            delta(out)
         return self.all_reduce(out)
 
     def gather_logits(self, local_logits: torch.Tensor, vocab_size: int) -> torch.Tensor:

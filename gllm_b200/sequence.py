@@ -11,14 +11,14 @@ class Sequence:
                  "mm_contents", "page_hashes", "num_cached_tokens", "arrival_time", "first_token_time",
                  "finish_time", "slot", "mrope_delta", "mm_state", "pt_np", "pending", "zombie", "pt_gen", "published",
                  "slot_fresh", "logprobs", "output_logprobs", "seed", "frequency_penalty", "presence_penalty",
-                 "logit_bias", "forks", "prompt_logprobs_n", "plp_cursor", "prompt_logprobs")
+                 "logit_bias", "forks", "prompt_logprobs_n", "plp_cursor", "prompt_logprobs", "lora_id")
 
     def __init__(self, seq_id: int, token_ids: List[int], finish_tokens: List[int],
                  output_len: Optional[int] = None, ignore_eos: bool = False, temperature: float = 0.6,
                  top_p: float = 0.9, top_k: int = 10, repetition_penalty: float = 1.0, mm_contents=None,
                  logprobs: int = -1, seed: Optional[int] = None, frequency_penalty: float = 0.0,
                  presence_penalty: float = 0.0, logit_bias: Optional[Dict[int, float]] = None,
-                 prompt_logprobs: int = -1):
+                 prompt_logprobs: int = -1, lora_id: int = 0):
         self.seq_id = seq_id
         self.token_ids: List[int] = list(token_ids)
         self.prompt_len = len(self.token_ids)
@@ -76,6 +76,8 @@ class Sequence:
         # and are not scheduled on their own: when its final prompt chunk is scheduled they take its full prompt
         # pages, a copy of its partial last page, and first tokens drawn from its last logits row. Emptied then.
         self.forks: List["Sequence"] = []
+        # multi-LoRA: the adapter this request runs with (0: the base model; adapter i has device slot i - 1)
+        self.lora_id = lora_id
 
     @property
     def plp_pending(self) -> bool:
