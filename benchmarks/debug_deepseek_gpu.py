@@ -4,7 +4,6 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from gllm_b200 import LLM
 from gllm_b200.models import deepseek_v2 as ds
-from gllm_b200.ops import ref
 
 cfg = {"architectures": ["DeepseekV3ForCausalLM"], "hidden_size": 256, "intermediate_size": 512,
        "moe_intermediate_size": 128, "num_hidden_layers": 3, "num_attention_heads": 8, "num_key_value_heads": 8,
@@ -47,8 +46,6 @@ for vname, v in VARIANTS.items():
             params = [(n, p.detach().cpu().clone()) for n, p in model.named_parameters()]
         else:
             for (n, p), (n2, q) in zip(model.named_parameters(), params):
-                if n.endswith("experts.w13"):
-                    q = torch.stack([ref.interleave_gate_up(q[e], 64) for e in range(q.shape[0])])
                 p.data.copy_(q.to(p.device))
             model.process_weights()
         rec[dev] = []

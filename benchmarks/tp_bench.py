@@ -17,7 +17,7 @@ def main():
     torch.cuda.set_device(local)
     from gllm_b200.parallel import state as ps
     ps.init_dist(1, world, rank, local)
-    from gllm_b200.ops import ref
+    from gllm_b200.ops import ref, sm100
     from gllm_b200.parallel.fused import FusedTPComm
     from gllm_b200.parallel.tp import TPComm
     dev = torch.device("cuda", local)
@@ -29,7 +29,7 @@ def main():
     w_qkv = (torch.randn(QKV, H, device=dev) * 0.02).bfloat16()
     nw = torch.ones(H, device=dev).bfloat16()
     fused = FusedTPComm(max_tokens=8192, hidden_size=H, device=dev)
-    base = TPComm()
+    base = TPComm(sm100)
 
     def block(tpc, a, res):
         h, res = tpc.row_linear_add_norm(a, w_o, res, nw, 1e-6)

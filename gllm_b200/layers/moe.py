@@ -17,7 +17,7 @@ from typing import Optional
 import torch
 from torch import nn
 
-from gllm_b200.layers import functional as Fn
+from gllm_b200 import ops
 from gllm_b200.models import weight_utils as wu
 from gllm_b200.ops import ref
 from gllm_b200.parallel import state as ps
@@ -33,6 +33,7 @@ class FusedMoE(nn.Module):
                  n_group: int = 0, topk_group: int = 0, routed_scaling: float = 1.0, bias_correction: bool = False,
                  quant: Optional[str] = None):
         super().__init__()
+        self.ops = ops.table(device)
         self.quant = quant if (quant == "fp8" and hidden % 128 == 0) else None
         st = ps.get_state()
         self.num_experts, self.top_k, self.hidden = num_experts, top_k, hidden
@@ -75,7 +76,7 @@ class FusedMoE(nn.Module):
     def process_weights(self):
         """The wgmma GEMM wants N % 8 == 0: expert counts like 60 (Qwen1.5-MoE) get a zero-padded router
         weight, built once after loading (before CUDA-graph capture); the logits are sliced back to E columns."""
-        if self.router_w.is_cuda and self.num_experts % 8 != 0:
+        if self.num_experts % 8 != 0:
             e_pad = (self.num_experts + 7) // 8 * 8
             old = getattr(self, "_router_pad", None)
             if old is None:
@@ -84,38 +85,26 @@ class FusedMoE(nn.Module):
             old[: self.num_experts].copy_(self.router_w.data)
 
     def _router_logits(self, h: torch.Tensor) -> torch.Tensor:
-        if h.is_cuda and self.num_experts % 8 != 0:
+        if self.num_experts % 8 != 0:
             if getattr(self, "_router_pad", None) is None:
-                assert not torch.cuda.is_current_stream_capturing(), "call model.process_weights() before capture"
+                assert not (torch.cuda.is_available() and torch.cuda.is_current_stream_capturing()), \
+                    "call model.process_weights() before capture"
                 self.process_weights()
-            return Fn.linear(h, self._router_pad)[:, : self.num_experts]
-        return Fn.linear(h, self.router_w)
+            return self.ops.linear(h, self._router_pad)[:, : self.num_experts]
+        return self.ops.linear(h, self.router_w)
 
     def route(self, h: torch.Tensor):
         logits = self._router_logits(h)
         if self.n_group > 0:
-            return ref.grouped_topk(logits, self.top_k, self.renormalize, self.n_group, self.topk_group,
-                                    self.scoring, self.e_bias, self.routed_scaling) if not h.is_cuda else \
-                _sm_grouped_topk(self, logits)
-        if h.is_cuda:
-            from gllm_b200.ops import sm100_moe
-            return sm100_moe.topk_softmax(logits, self.top_k, self.renormalize)
-        return ref.topk_softmax(logits, self.top_k, self.renormalize)
+            return self.ops.grouped_topk(logits, self.top_k, self.renormalize, self.n_group, self.topk_group,
+                                         self.scoring, self.e_bias, self.routed_scaling)
+        return self.ops.topk_softmax(logits, self.top_k, self.renormalize)
 
     def forward(self, h: torch.Tensor, tpc=None) -> torch.Tensor:
         w, ids = self.route(h)
         if self.quant == "fp8":
-            if h.is_cuda:
-                from gllm_b200.ops import sm100_moe
-                return sm100_moe.fused_experts_fp8(h, self.w13, self.w13_ws, self.w2, self.w2_ws, w, ids,
-                                                   self.expert_map)
-            w13 = (self.w13.float() * self.w13_ws.repeat_interleave(64, 1).repeat_interleave(128, 2)).to(h.dtype)
-            w2 = (self.w2.float() * self.w2_ws.repeat_interleave(64, 1).repeat_interleave(128, 2)).to(h.dtype)
-            return ref.fused_experts(h, w13, w2, w, ids, self.expert_map)
-        if h.is_cuda:
-            from gllm_b200.ops import sm100_moe
-            return sm100_moe.fused_experts(h, self.w13, self.w2, w, ids, self.expert_map)
-        return ref.fused_experts(h, self.w13, self.w2, w, ids, self.expert_map)
+            return self.ops.fused_experts_fp8(h, self.w13, self.w13_ws, self.w2, self.w2_ws, w, ids, self.expert_map)
+        return self.ops.fused_experts(h, self.w13, self.w2, w, ids, self.expert_map)
 
     # -- weights ----------------------------------------------------------------------------------
     def load_expert(self, global_e: int, gate: torch.Tensor, up: torch.Tensor, down: torch.Tensor):
@@ -128,44 +117,24 @@ class FusedMoE(nn.Module):
         else:
             gu = wu.shard_gate_up(gate, up, self.tp_rank, self.tp_size)
             down = wu.shard_cols(down, self.tp_rank, self.tp_size)
+        # w13: gate/up rows interleaved as the grouped GEMM's SiLU-gate epilogue reads them (fp8: I % 128 == 0)
         if self.quant == "fp8":
             q13, s13 = _block_quant_rows64(gu)
             q2, s2 = _block_quant_rows64(down)
-            if self.w13.is_cuda:
-                q13 = ref.interleave_gate_up(q13.view(torch.uint8), 64).view(torch.float8_e4m3fn)
-                s13 = ref.interleave_gate_up(s13, 1)
-            self.w13.data[le].copy_(q13)
-            self.w13_ws.data[le].copy_(s13)
+            self.w13.data[le].copy_(ref.interleave_gate_up(q13.view(torch.uint8), 64).view(torch.float8_e4m3fn))
+            self.w13_ws.data[le].copy_(ref.interleave_gate_up(s13, 1))
             self.w2.data[le].copy_(q2)
             self.w2_ws.data[le].copy_(s2)
             return
-        if self.w13.is_cuda:
-            # the grouped GEMM's SiLU-gate epilogue wants gate/up rows interleaved per 64
-            assert self.inter % 64 == 0, "sm_90a MoE path needs intermediate % 64 == 0"
-            gu = ref.interleave_gate_up(gu, 64)
-        self.w13.data[le].copy_(gu)
+        self.w13.data[le].copy_(ref.interleave_gate_up(gu, ref.moe_gate_up_block(self.inter)))
         self.w2.data[le].copy_(down)
 
 
 def _block_quant_rows64(w: torch.Tensor):
-    """[N, K] -> (e4m3 [N, K], fp32 scales [N/64, K/128]): 128x128 block quantisation (scale = amax / 448) of
-    the checkpoint layout, scales repeated per 64-row half block. Lossless for a de-quantised fp8 checkpoint
-    whose blocks are aligned (N, K multiples of 128)."""
-    w = w.float()
-    n, k = w.shape
-    nb, kb = (n + 127) // 128, (k + 127) // 128
-    wp = torch.zeros(nb * 128, kb * 128, dtype=torch.float32, device=w.device)
-    wp[:n, :k] = w
-    blk = wp.view(nb, 128, kb, 128)
-    sc = (blk.abs().amax(dim=(1, 3)) / 448.0).clamp_min(1e-12)
-    q = (blk / sc.view(nb, 1, kb, 1)).view(nb * 128, kb * 128)[:n, :k].to(torch.float8_e4m3fn)
-    return q, sc.repeat_interleave(2, 0)[: (n + 63) // 64]
-
-
-def _sm_grouped_topk(moe: FusedMoE, logits):
-    from gllm_b200.ops import sm100_moe
-    return sm100_moe.grouped_topk(logits, moe.top_k, moe.renormalize, moe.n_group, moe.topk_group, moe.scoring,
-                                  moe.e_bias, moe.routed_scaling)
+    """[N, K] -> (e4m3 [N, K], fp32 scales [N/64, K/128]): `weight_utils.fp8_block_quant` with the scales
+    repeated per 64-row half block, so that an interleaved [64 gate | 64 up] GEMM tile carries two block scales."""
+    q, sc = wu.fp8_block_quant(w)
+    return q, sc.repeat_interleave(2, 0)[: (w.shape[0] + 63) // 64]
 
 
 class SparseMoeBlock(nn.Module):
@@ -191,7 +160,7 @@ class SparseMoeBlock(nn.Module):
         if self.shared is not None:
             # partial (un-reduced) shared-expert output: reduced together with the routed experts —
             # the reference double-reduces here on Qwen2-MoE (SURVEY §2.2 C23); we do it once.
-            s = Fn.linear(self.shared.act(h, tpc), self.shared.down_weight())
+            s = self.experts.ops.linear(self.shared.act(h, tpc), self.shared.down_weight())
             if self.shared_gate_w is not None:
                 g = torch.sigmoid(torch.nn.functional.linear(h.float(), self.shared_gate_w.float()))
                 s = (s.float() * g).to(s.dtype)

@@ -24,7 +24,7 @@ from typing import Dict, List, Optional, Tuple
 
 import torch
 
-from gllm_b200.layers import functional as Fn
+from gllm_b200 import ops
 from gllm_b200.models import weight_utils as wu
 from gllm_b200.ops import ref
 
@@ -141,20 +141,22 @@ def load_adapter(path: str, spec, max_lora_rank: int) -> Dict[Tuple[int, str], T
 class LoraLayer:
     """One decoder layer's stacked adapter weights on this rank, and the three ways the forward applies them."""
 
-    def __init__(self, tensors: Dict[str, torch.Tensor], bounds: Dict[str, List[int]], fused_act: bool):
+    def __init__(self, tensors: Dict[str, torch.Tensor], bounds: Dict[str, List[int]], fused_act: bool, device):
         self.t = tensors           # "<group>_A" [L, m·R, K_local], "<group>_B" [L, N_local, R]
         self.bounds = bounds       # group -> column offsets of its modules in the output
         self.fused_act = fused_act
+        self.ops = ops.table(device)
 
     def add(self, group: str, csr, x: torch.Tensor, y: torch.Tensor):
-        """y += delta of `group` (qkv, gate_up, o, down) for the adapter rows of input x, in place."""
-        u = Fn.lora_shrink(x, self.t[group + "_A"], csr)
-        Fn.lora_expand_add(y, u, self.t[group + "_B"], self.bounds[group], csr)
+        """y += delta of `group` (qkv, gate_up, o, down) for the adapter rows of input x, in place. `csr`: the batch's
+        (slots, row offsets, rows, number of groups), `InputData.lora`."""
+        u = self.ops.lora_shrink(x, self.t[group + "_A"], *csr)
+        self.ops.lora_expand_add(y, u, self.t[group + "_B"], self.bounds[group], *csr)
 
     def silu_mul(self, csr, x: torch.Tensor, pre: torch.Tensor) -> torch.Tensor:
         """Interleaved gate/up pre-activations of the fused-act layout -> SiLU(gate + dg) · (up + du)."""
-        u = Fn.lora_shrink(x, self.t["gate_up_A"], csr)
-        return Fn.lora_expand_silu_mul(pre, u, self.t["gate_up_B"], csr)
+        u = self.ops.lora_shrink(x, self.t["gate_up_A"], *csr)
+        return self.ops.lora_expand_silu_mul(pre, u, self.t["gate_up_B"], *csr)
 
 
 class LoraStore:
@@ -202,4 +204,4 @@ class LoraStore:
             qs, kvs, inter = at.q_size, at.kv_size, mlp.inter
             bounds = {"qkv": [0, qs, qs + kvs, qs + 2 * kvs], "gate_up": [0, inter, 2 * inter],
                       "o": [0, spec.hidden_size], "down": [0, spec.hidden_size]}
-            layer.lora = LoraLayer(stacked, bounds, mlp.fused_act)
+            layer.lora = LoraLayer(stacked, bounds, mlp.fused_act, device)

@@ -146,10 +146,10 @@ class ModelRunner:
             "LoRA adapters" if cfg.lora_modules else None
         if want_fused and why_not:
             logger.warning("tp_mode=fused is not available with %s: tensor-parallel collectives run on NCCL", why_not)
-        self.tpc = make_tp_comm(fused=(want_fused and why_not is None),
+        self.tpc = make_tp_comm(self.device, fused=(want_fused and why_not is None),
                                 max_tokens=self.max_num_batched_tokens,
-                                hidden_size=self.spec.hidden_size, dtype=self.spec.dtype, device=self.device) \
-            if cfg.tp_size > 1 else make_tp_comm(False)
+                                hidden_size=self.spec.hidden_size, dtype=self.spec.dtype) \
+            if cfg.tp_size > 1 else make_tp_comm(self.device)
         max_blocks = (self.model_max_length + self.page_size - 1) // self.page_size + 1
         mrope = self.model.rope.mrope_section is not None if hasattr(self.model, "rope") else False
         self.input_data = InputData(self.max_num_batched_tokens, max(self.max_running_seqs, 1), max_blocks,

@@ -21,7 +21,7 @@ from typing import Callable, Dict, List, Optional
 import torch
 from torch import nn
 
-from gllm_b200.layers import functional as Fn
+from gllm_b200 import ops
 from gllm_b200.layers.rotary import RopeSpec, build_rope
 from gllm_b200.models import weight_utils as wu
 from gllm_b200.ops import ref
@@ -123,20 +123,12 @@ def _qw(w, s):
 
 
 def _store_linear(w_param, s_param, w: torch.Tensor):
-    """Copy a (sharded) weight into its parameter; fp8 parameters are block-quantised here (128x128 blocks,
-    scale_inv = amax / 448). Re-quantising the de-quantised tensor of an fp8 checkpoint is lossless as long
-    as shard boundaries fall on block boundaries (they do: head_dim 128, intermediate % 128 == 0)."""
+    """Copy a (sharded) weight into its parameter; fp8 parameters are block-quantised here
+    (`weight_utils.fp8_block_quant`)."""
     if s_param is None:
         w_param.data.copy_(w)
         return
-    w = w.float()
-    n, k = w.shape
-    nb, kb = (n + 127) // 128, (k + 127) // 128
-    wp = torch.zeros(nb * 128, kb * 128, dtype=torch.float32, device=w.device)
-    wp[:n, :k] = w
-    blk = wp.view(nb, 128, kb, 128)
-    sc = (blk.abs().amax(dim=(1, 3)) / 448.0).clamp_min(1e-12)
-    q = (blk / sc.view(nb, 1, kb, 1)).view(nb * 128, kb * 128)[:n, :k].to(torch.float8_e4m3fn)
+    q, sc = wu.fp8_block_quant(w)
     w_param.data.copy_(q)
     s_param.data.copy_(sc)
 
@@ -146,6 +138,7 @@ class Attention(nn.Module):
         super().__init__()
         st = ps.get_state()
         tp, tr = st.tp_size, st.tp_rank
+        self.ops = ops.table(device)
         self.layer_id = layer_id
         self.head_dim = spec.head_dim
         assert spec.num_heads % tp == 0, f"{spec.num_heads} heads not divisible by tp={tp}"
@@ -185,16 +178,21 @@ class Attention(nn.Module):
             # memory-profiling run without a KV cache (reference: gllm/layers/attention.py:34-36)
             return qkv[:, : self.q_size].contiguous()
         kc, vc = kv_cache.k_cache[self.layer_id], kv_cache.v_cache[self.layer_id]
-        Fn.rope_kv_write(q, k, v, inp.positions, self.rope.cos_sin, self.rope.rot_dim, self.rope.neox,
-                         self.q_norm_w, self.k_norm_w, self.eps, kc, vc, inp.slot_mapping,
-                         self.rope.mrope_section)
-        return Fn.paged_attention(qkv[:, : self.q_size], kc, vc, inp, self.scaling, self.num_heads, d)
+        self.ops.rope_kv_write(q, k, v, inp.positions, self.rope.cos_sin, self.rope.rot_dim, self.rope.neox,
+                               self.q_norm_w, self.k_norm_w, self.eps, kc, vc, inp.slot_mapping,
+                               self.rope.mrope_section)
+        # a CUDA-graph batch padded to `padded_tokens` rows runs every row as a decode sequence
+        return self.ops.paged_attention(qkv[:, : self.q_size], kc, vc, inp.block_table, inp.seq_lens,
+                                        inp.query_start_loc, self.scaling, self.num_heads, d,
+                                        inp.padded_tokens or inp.num_decode_seqs, inp.padded_tokens or inp.num_seqs,
+                                        inp.max_q_len, inp.max_seq_len, splits=inp.decode_splits)
 
 
 class DenseMLP(nn.Module):
     def __init__(self, hidden: int, intermediate: int, dtype, device, shard: bool = True,
                  spec: Optional[ModelSpec] = None):
         super().__init__()
+        self.ops = ops.table(device)
         tp = ps.get_tp_size() if shard else 1
         assert intermediate % tp == 0
         self.inter = intermediate // tp
@@ -224,10 +222,10 @@ class DenseMLP(nn.Module):
                 return lora.silu_mul(csr, h, tpc.col_linear(h, self.gate_up_w))
             pre = tpc.col_linear(h, _qw(self.gate_up_w, self.gate_up_ws))
             lora.add("gate_up", csr, h, pre)
-            return Fn.silu_and_mul(pre)
+            return self.ops.silu_and_mul(pre)
         if self.fused_act:
             return tpc.col_linear_silu_mul(h, self.gate_up_w)
-        return Fn.silu_and_mul(tpc.col_linear(h, _qw(self.gate_up_w, self.gate_up_ws)))
+        return self.ops.silu_and_mul(tpc.col_linear(h, _qw(self.gate_up_w, self.gate_up_ws)))
 
 
 class DecoderLayer(nn.Module):
@@ -283,6 +281,7 @@ class CausalLM(nn.Module):
         self.spec = spec
         st = ps.get_state()
         self.device = torch.device(device)
+        self.ops = ops.table(device)
         self.layers_range = ps.get_pp_layers(spec.num_layers)
         self.is_first, self.is_last = ps.is_first_pp_rank(), ps.is_last_pp_rank()
         self.tp_size, self.tp_rank = st.tp_size, st.tp_rank
@@ -319,7 +318,7 @@ class CausalLM(nn.Module):
 
     # -- forward ----------------------------------------------------------------------------------
     def embed(self, inp, tpc: TPComm) -> torch.Tensor:
-        x = Fn.embedding(inp.tokens, self.embed_w, self.vocab_start, self.vocab_start + self.vocab_per_rank)
+        x = self.ops.embedding(inp.tokens, self.embed_w, self.vocab_start, self.vocab_start + self.vocab_per_rank)
         return tpc.all_reduce(x)
 
     def forward(self, inp, kv_cache, tpc: TPComm, hidden: Optional[torch.Tensor] = None,
@@ -351,7 +350,7 @@ class CausalLM(nn.Module):
                     for _, _, works in recv_tiles:
                         for w in works:
                             w.wait()
-                _, res_full = Fn.rmsnorm(hidden, self.layers[0].input_norm_w, eps, residual)
+                _, res_full = self.ops.rmsnorm(hidden, self.layers[0].input_norm_w, eps, residual)
                 h, residual = tpc.first_norm(res_full, self.layers[0].input_norm_w, eps)
             elif recv_tiles and len(recv_tiles) > 1 and hasattr(self.layers[0].attn, "qkv_proj"):
                 # tile-streamed pipeline input: add+RMSNorm and the QKV GEMM run per row tile as the tiles
@@ -361,7 +360,7 @@ class CausalLM(nn.Module):
                 for r0, r1, works in recv_tiles:
                     for w in works:
                         w.wait()  # stream-level wait on this tile only
-                    Fn.rmsnorm(hidden[r0:r1], self.layers[0].input_norm_w, eps, residual[r0:r1], out=h[r0:r1])
+                    self.ops.rmsnorm(hidden[r0:r1], self.layers[0].input_norm_w, eps, residual[r0:r1], out=h[r0:r1])
                     q = at.qkv_proj(h[r0:r1], tpc)
                     if qkv0 is None:
                         qkv0 = torch.empty(hidden.shape[0], q.shape[1], dtype=q.dtype, device=q.device)
@@ -371,7 +370,7 @@ class CausalLM(nn.Module):
                     for _, _, works in recv_tiles:
                         for w in works:
                             w.wait()
-                h, residual = Fn.rmsnorm(hidden, self.layers[0].input_norm_w, eps, residual)
+                h, residual = self.ops.rmsnorm(hidden, self.layers[0].input_norm_w, eps, residual)
         nvtx = _NVTX and h.is_cuda
         for i, layer in enumerate(self.layers):
             if nvtx:
@@ -387,7 +386,7 @@ class CausalLM(nn.Module):
                 # visual token rows before the next block's norm (reference: models/qwen3_vl.py:525-568)
                 out, residual = layer(inp, h, residual, kv_cache, tpc, None)
                 out.index_add_(0, deepstack[0], deepstack[1][i])
-                h, residual = Fn.rmsnorm(out, nxt, eps, residual)
+                h, residual = self.ops.rmsnorm(out, nxt, eps, residual)
             elif i == 0 and qkv0 is not None:
                 h, residual = layer(inp, h, residual, kv_cache, tpc, nxt, qkv=qkv0)
             else:
@@ -400,14 +399,14 @@ class CausalLM(nn.Module):
 
     def lm_head(self, rows: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
         """This rank's vocab shard of the logits of final-normed hidden `rows` -> [R, Vp/tp] (into `out` if given)."""
-        return Fn.linear(rows, self.lm_head_w, out=out)
+        return self.ops.linear(rows, self.lm_head_w, out=out)
 
     def compute_logits(self, inp, hidden: torch.Tensor, tpc: TPComm, all_rows: bool = False,
                        local: bool = False) -> torch.Tensor:
         """Logits of the last token of every emitting sequence -> [E, V]; `local=True` returns this rank's vocab
         shard [E, Vp/tp] instead (vocab-parallel sampling: the runner reduces winners, not logits). `hidden` is the
         final-normed activation after `tpc.materialize`."""
-        rows = hidden if all_rows else Fn.gather_rows(hidden, inp.logits_idx)
+        rows = hidden if all_rows else self.ops.gather_rows(hidden.contiguous(), inp.logits_idx)
         shard = self.lm_head(rows)
         if local:
             return shard

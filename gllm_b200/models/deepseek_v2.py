@@ -22,7 +22,7 @@ import torch
 import torch.nn.functional as F
 from torch import nn
 
-from gllm_b200.layers import functional as Fn
+from gllm_b200 import ops
 from gllm_b200.layers.moe import SparseMoeBlock
 from gllm_b200.layers.rotary import build_rope
 from gllm_b200.models import weight_utils as wu
@@ -40,6 +40,7 @@ class MLAAttention(nn.Module):
         x = spec.extra
         st = ps.get_state()
         tp = st.tp_size
+        self.ops = ops.table(device)
         self.layer_id = layer_id
         self.tp, self.tr = tp, st.tp_rank
         self.num_heads = spec.num_heads // tp
@@ -73,17 +74,18 @@ class MLAAttention(nn.Module):
         hl = self.num_heads
         h = tpc.materialize(h)
         if self.q_lora:
-            qa, _ = Fn.rmsnorm(Fn.linear(h, _qw(self.q_a_w, self.q_a_ws)), self.q_a_norm_w, self.eps)
-            q = Fn.linear(qa, _qw(self.q_b_w, self.q_b_ws))
+            qa, _ = self.ops.rmsnorm(self.ops.linear(h, _qw(self.q_a_w, self.q_a_ws)), self.q_a_norm_w, self.eps)
+            q = self.ops.linear(qa, _qw(self.q_b_w, self.q_b_ws))
         else:
-            q = Fn.linear(h, _qw(self.q_w, self.q_ws))
+            q = self.ops.linear(h, _qw(self.q_w, self.q_ws))
         q = q.view(t, hl, self.qk_dim)
-        kv_a = Fn.linear(h, _qw(self.kv_a_w, self.kv_a_ws))
-        kv_c, _ = Fn.rmsnorm(kv_a[:, : self.kv_lora].contiguous(), self.kv_a_norm_w, self.eps)
+        kv_a = self.ops.linear(h, _qw(self.kv_a_w, self.kv_a_ws))
+        kv_c, _ = self.ops.rmsnorm(kv_a[:, : self.kv_lora].contiguous(), self.kv_a_norm_w, self.eps)
         if kv_cache is None:
             return q[:, :, : self.v_dim].reshape(t, hl * self.v_dim).contiguous()
         cache = kv_cache.k_cache[self.layer_id]
-        if h.is_cuda and self.kv_lora == 512 and self.rope_dim == 64:
+        # the absorbed kernels need kv_lora 512 / rope 64: the expanded form below serves every other shape
+        if self.ops is ops.sm100 and self.kv_lora == 512 and self.rope_dim == 64:
             return self._forward_absorbed(inp, q, kv_c, kv_a[:, self.kv_lora:], cache)
         k_pe = kv_a[:, self.kv_lora:].contiguous().view(t, 1, self.rope_dim)
         q_pe = q[:, :, self.nope:].contiguous()
@@ -140,18 +142,17 @@ class MLAAttention(nn.Module):
     def _forward_absorbed(self, inp, q, kv_c, k_pe, cache):
         """sm_90a path: multi-query attention over the latent cache (csrc/attn/mla_attention.cu). No host
         synchronisation, so decode batches run inside CUDA graphs."""
-        from gllm_b200.ops import sm100
         t, hl = q.shape[0], self.num_heads
         w_uk, w_uv = self._absorbed_weights()
         q_full = torch.empty(t, hl, 576, dtype=q.dtype, device=q.device)
-        sm100.gemm_batched(q[:, :, : self.nope], w_uk, q_full[:, :, :512])   # per head: q_nope · W_UK
-        sm100.mla_rope_cache(q[:, :, self.nope:], q_full, k_pe, kv_c, self.rope.cos_sin, inp.positions,
-                             inp.slot_mapping, cache)
-        splits = sm100.mla_splits(t, hl)
-        out_lat = sm100.mla_attention(q_full, cache, inp.block_table, inp.tok_seq, inp.positions, self.scaling,
-                                      splits=splits)
+        self.ops.gemm_batched(q[:, :, : self.nope], w_uk, q_full[:, :, :512])   # per head: q_nope · W_UK
+        self.ops.mla_rope_cache(q[:, :, self.nope:], q_full, k_pe, kv_c, self.rope.cos_sin, inp.positions,
+                                inp.slot_mapping, cache)
+        splits = self.ops.mla_splits(t, hl)
+        out_lat = self.ops.mla_attention(q_full, cache, inp.block_table, inp.tok_seq, inp.positions, self.scaling,
+                                         splits=splits)
         out = torch.empty(t, hl, self.v_dim, dtype=q.dtype, device=q.device)
-        sm100.gemm_batched(out_lat, w_uv, out)                                # per head: out_lat · W_UV
+        self.ops.gemm_batched(out_lat, w_uv, out)                               # per head: out_lat · W_UV
         return out.view(t, hl * self.v_dim)
 
 
@@ -189,6 +190,7 @@ class DeepseekForCausalLM(CausalLM):
         self.spec = spec
         st = ps.get_state()
         self.device = torch.device(device)
+        self.ops = ops.table(device)
         self.layers_range = ps.get_pp_layers(spec.num_layers)
         self.is_first, self.is_last = ps.is_first_pp_rank(), ps.is_last_pp_rank()
         self.tp_size, self.tp_rank = st.tp_size, st.tp_rank

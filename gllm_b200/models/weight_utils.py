@@ -81,6 +81,21 @@ def expert_range(num_experts: int, ep_rank: int, ep_size: int):
     return start, n
 
 
+def fp8_block_quant(w: torch.Tensor):
+    """[N, K] -> (e4m3 [N, K], fp32 scale_inv [ceil(N/128), ceil(K/128)]): 128x128 block quantisation, scale_inv =
+    amax / 448 per block. Re-quantising the de-quantised tensor of an fp8 checkpoint is lossless as long as the
+    blocks stay aligned (shard boundaries on block boundaries: head_dim 128, intermediate % 128 == 0)."""
+    w = w.float()
+    n, k = w.shape
+    nb, kb = (n + 127) // 128, (k + 127) // 128
+    wp = torch.zeros(nb * 128, kb * 128, dtype=torch.float32, device=w.device)
+    wp[:n, :k] = w
+    blk = wp.view(nb, 128, kb, 128)
+    sc = (blk.abs().amax(dim=(1, 3)) / 448.0).clamp_min(1e-12)
+    q = (blk / sc.view(nb, 1, kb, 1)).view(nb * 128, kb * 128)[:n, :k].to(torch.float8_e4m3fn)
+    return q, sc
+
+
 # ------------------------------------------------------------------------------------------------
 # checkpoint reader
 # ------------------------------------------------------------------------------------------------

@@ -1,7 +1,8 @@
-"""CPU stand-ins for the sampler ops of `ops.sm100`, with the same signatures and the same device-state formats:
-seen-token bitmask rows plus a slot index, per-slot bias rows plus a slot, and an RNG keyed by `seed` plus the step
-counter. Each stand-in converts that state to the dense arguments of its `ops.ref` oracle. This is the CPU plumbing
-path only; it never stands in for a missing kernel on a GPU.
+"""CPU stand-ins for the ops of `ops.sm100` that the model forward and the sampler call, with the same signatures, the
+same weight layouts and `out=` / in-place contracts, and the same device-state formats: seen-token bitmask rows plus a
+slot index, per-slot bias rows plus a slot, and an RNG keyed by `seed` plus the step counter. Each stand-in converts
+that state to the dense arguments of its `ops.ref` oracle. This is the CPU plumbing path only; it never stands in for a
+missing kernel on a GPU.
 """
 from __future__ import annotations
 
@@ -10,9 +11,98 @@ from typing import Optional
 import torch
 
 from gllm_b200.ops import ref
-from gllm_b200.ops.ref import (kv_copy_pages, logprobs_final, logprobs_shard,  # noqa: F401  (sm100 signatures)
-                               prompt_logprobs_shard)
+from gllm_b200.ops.lib import GemmComm
+from gllm_b200.ops.ref import (grouped_topk, kv_copy_pages, logprobs_final,  # noqa: F401  (sm100 signatures)
+                               logprobs_shard, prompt_logprobs_shard, rope_kv_write, topk_softmax)
 from gllm_b200.parallel import state as ps
+
+
+def _into(out: Optional[torch.Tensor], y: torch.Tensor) -> torch.Tensor:
+    """`y`, or `out` holding it (the kernels' `out=` contract)."""
+    return y if out is None else out.copy_(y)
+
+
+def linear(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None,
+           out: Optional[torch.Tensor] = None, comm: Optional[GemmComm] = None, epi: int = 0) -> torch.Tensor:
+    assert comm is None and epi == 0, "GEMM epilogues over peer memory are sm_90a only"
+    if isinstance(w, tuple):
+        return linear_fp8_block(x, w[0], w[1], bias, out=out)
+    return _into(out, ref.linear(x, w, bias))
+
+
+def linear_silu_mul(x: torch.Tensor, w_interleaved: torch.Tensor, out: Optional[torch.Tensor] = None,
+                    comm: Optional[GemmComm] = None):
+    assert comm is None, "GEMM epilogues over peer memory are sm_90a only"
+    return _into(out, ref.linear_silu_mul(x, w_interleaved))
+
+
+def linear_fp8_block(x: torch.Tensor, w8: torch.Tensor, w_scale_inv: torch.Tensor,
+                     bias: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    return _into(out, ref.linear_fp8_block(x, w8, w_scale_inv, bias))
+
+
+def rmsnorm(x: torch.Tensor, w: torch.Tensor, eps: float, residual: Optional[torch.Tensor] = None,
+            out: Optional[torch.Tensor] = None, residual_out: Optional[torch.Tensor] = None):
+    o, r = ref.rmsnorm(x, w, eps, residual)
+    if residual is not None:
+        r = (residual if residual_out is None else residual_out).copy_(r)   # in place by default, as the kernel
+    return _into(out, o), r
+
+
+def silu_and_mul(x: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    return _into(out, ref.silu_and_mul(x))
+
+
+def embedding(ids: torch.Tensor, table: torch.Tensor, vocab_start: int = 0, vocab_end: Optional[int] = None,
+              out: Optional[torch.Tensor] = None):
+    return _into(out, ref.embedding(ids, table, vocab_start, vocab_end))
+
+
+def gather_rows(src: torch.Tensor, idx: torch.Tensor, out: Optional[torch.Tensor] = None):
+    return _into(out, src[idx.long()])
+
+
+def paged_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, block_table: torch.Tensor,
+                    seq_lens: torch.Tensor, query_start_loc: torch.Tensor, scale: float, num_q_heads: int,
+                    head_dim: int, num_decode_seqs: int, num_seqs: int, max_q_len: int, max_seq_len: int,
+                    out: Optional[torch.Tensor] = None, splits: Optional[int] = None) -> torch.Tensor:
+    """The decode / prefill split and its sizes only schedule the kernels: the oracle walks every sequence."""
+    return _into(out, ref.paged_attention(q, k_cache, v_cache, block_table, seq_lens, query_start_loc, scale,
+                                          num_q_heads, head_dim))
+
+
+def lora_shrink(x: torch.Tensor, A: torch.Tensor, slots: torch.Tensor, row_off: torch.Tensor, rows: torch.Tensor,
+                num_groups: int) -> torch.Tensor:
+    return ref.lora_shrink(x, A, slots, row_off, rows)
+
+
+def lora_expand_add(y: torch.Tensor, u: torch.Tensor, B: torch.Tensor, bounds, slots: torch.Tensor,
+                    row_off: torch.Tensor, rows: torch.Tensor, num_groups: int) -> torch.Tensor:
+    return ref.lora_expand_add(y, u, B, bounds, slots, row_off, rows)
+
+
+def lora_expand_silu_mul(pre: torch.Tensor, u: torch.Tensor, B: torch.Tensor, slots: torch.Tensor,
+                         row_off: torch.Tensor, rows: torch.Tensor, num_groups: int) -> torch.Tensor:
+    return ref.lora_expand_silu_mul(pre, u, B, slots, row_off, rows)
+
+
+def fused_experts(x: torch.Tensor, w13: torch.Tensor, w2: torch.Tensor, topk_w: Optional[torch.Tensor],
+                  topk_ids: torch.Tensor, expert_map: Optional[torch.Tensor] = None,
+                  out: Optional[torch.Tensor] = None, n_valid: Optional[torch.Tensor] = None,
+                  row_dest_fn=None) -> Optional[torch.Tensor]:
+    """w13 [E_local, 2I, H] with gate/up rows interleaved as the grouped GEMM reads them (`ref.moe_gate_up_block`)."""
+    assert n_valid is None and row_dest_fn is None, "the EP receive pool and peer-memory stores are sm_90a only"
+    block = ref.moe_gate_up_block(w13.shape[1] // 2)
+    return _into(out, ref.fused_experts(x, w13, w2, topk_w, topk_ids, expert_map, block=block))
+
+
+def fused_experts_fp8(x: torch.Tensor, w13: torch.Tensor, w13_s: torch.Tensor, w2: torch.Tensor, w2_s: torch.Tensor,
+                      topk_w: torch.Tensor, topk_ids: torch.Tensor, expert_map: Optional[torch.Tensor] = None,
+                      out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The experts de-quantised (scales per 64 weight rows and 128 columns), then `fused_experts`."""
+    def dq(w, s):
+        return (w.float() * s.repeat_interleave(64, 1).repeat_interleave(128, 2)).to(x.dtype)
+    return fused_experts(x, dq(w13, w13_s), dq(w2, w2_s), topk_w, topk_ids, expert_map, out)
 
 
 def _generator(seed: int, step: Optional[torch.Tensor], salt: int = 0) -> torch.Generator:

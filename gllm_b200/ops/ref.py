@@ -86,6 +86,12 @@ def interleave_gate_up(w: torch.Tensor, block: int = 128) -> torch.Tensor:
     return torch.cat([g, u], dim=1).reshape(two_i, k).contiguous()
 
 
+def moe_gate_up_block(inter: int) -> int:
+    """Rows per gate / up block of the MoE experts' w13 [E, 2I, H]: 64, the SiLU-gate tile of the grouped GEMM (which
+    needs I % 64 == 0); any other I, which only the CPU runs, keeps one block: the plain [gate; up] layout."""
+    return 64 if inter % 64 == 0 else inter
+
+
 def linear_silu_mul(x: torch.Tensor, w_interleaved: torch.Tensor, block: int = 128) -> torch.Tensor:
     y = F.linear(x, w_interleaved)
     t, two_i = y.shape
@@ -534,30 +540,29 @@ def logprobs_final(gathered: torch.Tensor, n: int) -> torch.Tensor:
 # ----------------------------------------------------------------------------------------------
 # MoE
 # ----------------------------------------------------------------------------------------------
-def topk_softmax(gate_logits: torch.Tensor, top_k: int, renormalize: bool):
-    probs = torch.softmax(gate_logits.float(), dim=-1)
+def topk_softmax(logits: torch.Tensor, top_k: int, renormalize: bool):
+    probs = torch.softmax(logits.float(), dim=-1)
     w, ids = torch.topk(probs, top_k, dim=-1)
     if renormalize:
         w = w / w.sum(-1, keepdim=True)
     return w, ids.to(torch.int32)
 
 
-def grouped_topk(gate_logits: torch.Tensor, top_k: int, renormalize: bool, num_groups: int,
-                 topk_group: int, scoring: str = "softmax", bias: Optional[torch.Tensor] = None,
-                 routed_scaling: float = 1.0):
+def grouped_topk(logits: torch.Tensor, top_k: int, renormalize: bool, n_group: int, topk_group: int,
+                 scoring: str = "softmax", bias: Optional[torch.Tensor] = None, routed_scaling: float = 1.0):
     """DeepSeek group-limited routing (reference: gllm/layers/moe/topk.py:87-138)."""
-    x = gate_logits.float()
+    x = logits.float()
     scores = torch.softmax(x, -1) if scoring == "softmax" else torch.sigmoid(x)
     t, e = scores.shape
     sel = scores + bias.float().view(1, -1) if bias is not None else scores
-    grp = sel.view(t, num_groups, e // num_groups)
+    grp = sel.view(t, n_group, e // n_group)
     if bias is not None:
         gscore = grp.topk(2, dim=-1)[0].sum(-1)
     else:
         gscore = grp.max(-1)[0]
     gidx = gscore.topk(topk_group, dim=-1)[1]
     gmask = torch.zeros_like(gscore).scatter(1, gidx, 1.0)
-    mask = gmask.unsqueeze(-1).expand(t, num_groups, e // num_groups).reshape(t, e)
+    mask = gmask.unsqueeze(-1).expand(t, n_group, e // n_group).reshape(t, e)
     masked = sel.masked_fill(mask == 0, float("-inf"))
     ids = masked.topk(top_k, dim=-1)[1]
     w = scores.gather(1, ids)
@@ -567,9 +572,11 @@ def grouped_topk(gate_logits: torch.Tensor, top_k: int, renormalize: bool, num_g
 
 
 def fused_experts(x: torch.Tensor, w13: torch.Tensor, w2: torch.Tensor, topk_w: torch.Tensor,
-                  topk_ids: torch.Tensor, expert_map: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """x [T,H]; w13 [E_local, 2I, H]; w2 [E_local, H, I]; ids are GLOBAL expert ids, expert_map maps
-    global -> local (or -1). Non-local experts contribute zero (reference EP semantics)."""
+                  topk_ids: torch.Tensor, expert_map: Optional[torch.Tensor] = None,
+                  block: Optional[int] = None) -> torch.Tensor:
+    """x [T,H]; w13 [E_local, 2I, H] (gate rows then up rows, or with `block` interleaved per `block` rows, see
+    interleave_gate_up); w2 [E_local, H, I]; ids are GLOBAL expert ids, expert_map maps global -> local (or -1).
+    Non-local experts contribute zero (reference EP semantics)."""
     t, h = x.shape
     out = torch.zeros(t, h, dtype=torch.float32, device=x.device)
     e_local = w13.shape[0]
@@ -581,7 +588,7 @@ def fused_experts(x: torch.Tensor, w13: torch.Tensor, w2: torch.Tensor, topk_w: 
         if tok.numel() == 0:
             continue
         xe = x[tok]
-        hdn = silu_and_mul(F.linear(xe, w13[e]))
+        hdn = silu_and_mul(F.linear(xe, w13[e])) if block is None else linear_silu_mul(xe, w13[e], block)
         ye = F.linear(hdn, w2[e]).float()
         out.index_add_(0, tok, ye * topk_w[tok, slot].float().unsqueeze(-1))
     return out.to(x.dtype)

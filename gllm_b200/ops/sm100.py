@@ -70,7 +70,9 @@ def _linear_smallm(x, w, bias, out, silu: bool):
 
 def linear(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None,
            out: Optional[torch.Tensor] = None, comm: Optional[GemmComm] = None, epi: int = 0) -> torch.Tensor:
-    """y = x @ w.T (+ bias). x [M, K] (row stride arbitrary, unit inner stride), w [N, K]."""
+    """y = x @ w.T (+ bias). x [M, K] (row stride arbitrary, unit inner stride), w [N, K] or (e4m3, scale_inv)."""
+    if isinstance(w, tuple):
+        return linear_fp8_block(x, w[0], w[1], bias, out=out)
     assert x.dtype == _BF16 and w.dtype == _BF16, (x.dtype, w.dtype)
     assert x.dim() == 2 and w.dim() == 2 and x.shape[1] == w.shape[1], (x.shape, w.shape)
     assert x.stride(1) == 1 and w.stride(1) == 1
@@ -712,3 +714,7 @@ def lora_expand_silu_mul(pre: torch.Tensor, u: torch.Tensor, B: torch.Tensor, sl
           "lora_expand_silu_mul")
     _count()
     return out
+
+
+# the MoE front-ends, so that a model module sees one table (sm100_moe imports _count and _p, defined above)
+from gllm_b200.ops.sm100_moe import fused_experts, fused_experts_fp8, grouped_topk, topk_softmax  # noqa: E402,F401

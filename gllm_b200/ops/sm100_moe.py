@@ -76,6 +76,7 @@ def fused_experts(x: torch.Tensor, w13: torch.Tensor, w2: torch.Tensor, topk_w: 
     t, h = x.shape
     e_local, two_i, _ = w13.shape
     inter = two_i // 2
+    assert inter % 64 == 0, "the SiLU-gate epilogue reads gate/up rows interleaved per 64"
     k = topk_ids.shape[1]
     dev = x.device
     if out is None and row_dest_fn is None:

@@ -24,7 +24,6 @@ from typing import Optional
 import torch
 import torch.distributed as dist
 
-from gllm_b200.layers import functional as Fn
 from gllm_b200.ops import lib as _lib
 from gllm_b200.ops.lib import MAX_PEERS, GemmComm, check, stream_ptr
 from gllm_b200.parallel import state as ps
@@ -110,7 +109,8 @@ class FusedTPComm(TPComm):
     fused = True
 
     def __init__(self, max_tokens: int, hidden_size: int, dtype=torch.bfloat16, device=None, **_):
-        super().__init__()
+        from gllm_b200.ops import sm100
+        super().__init__(sm100)
         assert dtype == torch.bfloat16, "fused TP path is bf16"
         import torch.distributed._symmetric_memory as symm
         st = ps.get_state()

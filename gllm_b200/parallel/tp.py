@@ -19,14 +19,15 @@ from typing import Callable, Optional
 
 import torch
 
-from gllm_b200.layers import functional as Fn
+from gllm_b200 import ops as _ops
 from gllm_b200.parallel import state as ps
 
 
 class TPComm:
     fused = False
 
-    def __init__(self):
+    def __init__(self, ops):
+        self.ops = ops     # op table of this rank's device (`gllm_b200.ops.table`)
         st = ps.get_state()
         self.tp_size = st.tp_size
         self.tp_rank = st.tp_rank
@@ -37,7 +38,7 @@ class TPComm:
 
     def first_norm(self, x: torch.Tensor, norm_w: torch.Tensor, eps: float):
         """Embedding output -> (normed block input, residual stream)."""
-        h, _ = Fn.rmsnorm(x, norm_w, eps)
+        h, _ = self.ops.rmsnorm(x, norm_w, eps)
         return h, x
 
     def materialize(self, h: torch.Tensor) -> torch.Tensor:
@@ -49,10 +50,10 @@ class TPComm:
         return residual
 
     def col_linear(self, x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None) -> torch.Tensor:
-        return Fn.linear(x, w, bias)
+        return self.ops.linear(x, w, bias)
 
     def col_linear_silu_mul(self, x: torch.Tensor, w_interleaved: torch.Tensor) -> torch.Tensor:
-        return Fn.linear_silu_mul(x, w_interleaved)
+        return self.ops.linear_silu_mul(x, w_interleaved)
 
     def all_reduce(self, x: torch.Tensor) -> torch.Tensor:
         return ps.tp_all_reduce(x)
@@ -63,9 +64,9 @@ class TPComm:
         if self.tp_size > 1:
             ps.tp_all_reduce(partial)
         if residual is None:
-            normed, _ = Fn.rmsnorm(partial, norm_w, eps)
+            normed, _ = self.ops.rmsnorm(partial, norm_w, eps)
             return normed, partial
-        return Fn.rmsnorm(partial, norm_w, eps, residual)
+        return self.ops.rmsnorm(partial, norm_w, eps, residual)
 
     def moe_add_norm(self, block, h: torch.Tensor, residual: Optional[torch.Tensor], norm_w: torch.Tensor,
                      eps: float):
@@ -79,14 +80,14 @@ class TPComm:
                             delta: Optional[Callable[[torch.Tensor], None]] = None):
         """`delta(partial)` (LoRA) adds to this rank's partial GEMM output in place, before the sum over ranks."""
         # bias is added once (rank 0) like the reference (gllm/layers/linear.py:230-258)
-        partial = Fn.linear(x, w, bias if self.tp_rank == 0 else None)
+        partial = self.ops.linear(x, w, bias if self.tp_rank == 0 else None)
         if delta is not None:
             delta(partial)
         return self.reduce_add_norm(partial, residual, norm_w, eps)
 
     def row_linear(self, x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None,
                    delta: Optional[Callable[[torch.Tensor], None]] = None) -> torch.Tensor:
-        out = Fn.linear(x, w, bias if self.tp_rank == 0 else None)
+        out = self.ops.linear(x, w, bias if self.tp_rank == 0 else None)
         if delta is not None:
             delta(out)
         return self.all_reduce(out)
@@ -98,9 +99,9 @@ class TPComm:
         return ps.tp_all_gather_last_dim(local_logits)[:, :vocab_size]
 
 
-def make_tp_comm(fused: bool = False, **kw) -> TPComm:
+def make_tp_comm(device, fused: bool = False, **kw) -> TPComm:
     st = ps.get_state()
     if fused and st.tp_size > 1 and torch.cuda.is_available():
         from gllm_b200.parallel.fused import FusedTPComm
-        return FusedTPComm(**kw)
-    return TPComm()
+        return FusedTPComm(device=device, **kw)
+    return TPComm(_ops.table(device))

@@ -1,6 +1,5 @@
 """Token sampling on the last pipeline stage: the per-slot device state of the sampling parameters and the flow from
-one step's logits to its tokens and log-probabilities. The op table is chosen once: the sm_90a kernels (`ops.sm100`)
-on a CUDA device, their CPU stand-ins (`ops.cpu`) otherwise, called with the same arguments."""
+one step's logits to its tokens and log-probabilities, on the op table of the device (`ops.table`)."""
 from __future__ import annotations
 
 from typing import Optional
@@ -8,8 +7,8 @@ from typing import Optional
 import numpy as np
 import torch
 
+from gllm_b200 import ops
 from gllm_b200.input_data import BatchArrays, InputData
-from gllm_b200.layers import functional as Fn
 from gllm_b200.parallel import state as ps
 
 
@@ -28,11 +27,7 @@ class Sampler:
     def __init__(self, device: torch.device, vocab_size: int, seed: int, inp: InputData, stats: dict,
                  vocab_parallel: bool):
         """`vocab_parallel`: the logits are this TP rank's vocab shard, and no rank ever gathers the [E, V] logits."""
-        if device.type == "cuda":
-            from gllm_b200.ops import sm100 as ops
-        else:
-            from gllm_b200.ops import cpu as ops
-        self.ops = ops
+        self.ops = ops.table(device)
         self.device, self.vocab_size, self.seed, self.inp, self.stats = device, vocab_size, seed, inp, stats
         self.vocab_parallel = vocab_parallel
         self.seen_bits = None    # int32 [slots, ceil(V/32)]: prompt + output tokens under the repetition penalty
@@ -186,7 +181,7 @@ class Sampler:
         buf = None
         for a in range(0, q, tile_rows):
             b = min(q, a + tile_rows)
-            x = Fn.gather_rows(hidden, rows[a:b])
+            x = self.ops.gather_rows(hidden.contiguous(), rows[a:b])
             logits = lm_head(x, None if buf is None else buf[: b - a])
             if buf is None:
                 buf = logits

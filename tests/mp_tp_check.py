@@ -44,7 +44,7 @@ def main():
             print("[tp_check]", *a, flush=True)
     log("dist ready")
     fused = FusedTPComm(max_tokens=1024, hidden_size=H, device=dev)
-    base = TPComm()
+    base = TPComm(sm100)
     log("symmetric buffers ready")
     ok = True
     def op_level(T, tag=""):
