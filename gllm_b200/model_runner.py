@@ -141,7 +141,9 @@ class ModelRunner:
         self.model = self.loader.load_model(self.device, progress)
         self.spec = self.model.spec
         want_fused = cfg.tp_mode == "fused" and cfg.tp_size > 1 and is_cuda
-        why_not = "fp8 block-scaled linears" if getattr(self.spec, "quant", None) is not None else \
+        quant = getattr(self.spec, "quant", None)
+        why_not = {"fp8": "fp8 block-scaled linears", "awq": "AWQ int4 linears",
+                   "gptq": "GPTQ int4 linears"}.get(quant, quant) if quant is not None else \
             "DeepStack (Qwen3-VL) feature injection" if getattr(self.model, "num_deepstack", 0) else \
             "LoRA adapters" if cfg.lora_modules else None
         if want_fused and why_not:

@@ -75,7 +75,9 @@ class ModelSpec:
     names: Dict[str, str] = field(default_factory=dict)
     eos_token_id: Optional[object] = None
     extra: dict = field(default_factory=dict)
-    quant: Optional[str] = None  # "fp8": block-scaled e4m3 linears (HF quantization_config, 128x128 blocks)
+    quant: Optional[str] = None  # "fp8": block-scaled e4m3 linears (HF quantization_config, 128x128 blocks);
+    #                              "awq" / "gptq": int4 q/k/v/o/gate/up/down with group scales (`w4`)
+    w4: Optional[wu.W4Config] = None
 
     def is_moe_layer(self, layer_id: int) -> bool:
         if self.moe is None:
@@ -107,8 +109,30 @@ def _param(*shape, dtype, device, std=0.02, fill=None):
     return nn.Parameter(t, requires_grad=False)
 
 
+class W4Params(nn.Module):
+    """Group scales and zero points of an int4 linear (its codes are the `*_w` parameter beside it), in the device
+    layout of `ref.Int4Weight`."""
+
+    def __init__(self, n: int, k: int, cfg: wu.W4Config, device):
+        super().__init__()
+        if cfg.group_size != -1 and k % cfg.group_size:
+            raise ValueError(f"{cfg.method}: a linear's per-rank input width {k} is not a multiple of group_size "
+                             f"{cfg.group_size} (reduce tp_size)")
+        self.group_size = cfg.group_size if cfg.group_size != -1 else k
+        self.in_features = k
+        g, np_ = -(-k // self.group_size), -(-n // 16) * 16
+        self.scales = nn.Parameter(torch.zeros(g, n, dtype=torch.float16, device=device), requires_grad=False)
+        self.zeros = nn.Parameter(torch.zeros(g, np_, dtype=torch.uint8, device=device), requires_grad=False)
+
+
 def _linear_params(n: int, k: int, spec: ModelSpec, device):
-    """(weight, scale_inv | None): bf16 [n, k], or e4m3 [n, k] + fp32 block scales for fp8 checkpoints."""
+    """(weight, scale_inv | None): bf16 [n, k], or e4m3 [n, k] + fp32 block scales for fp8 checkpoints, or packed
+    int4 codes + `W4Params` for AWQ / GPTQ checkpoints."""
+    if spec.w4 is not None:
+        assert k % 32 == 0 and n % 8 == 0, (n, k)
+        w = nn.Parameter(torch.zeros(-(-n // 16) * 16, -(-k // ref.W4_BLOCK_K) * ref.W4_BLOCK_K // 8,
+                                     dtype=torch.int32, device=device), requires_grad=False)
+        return w, W4Params(n, k, spec.w4, device)
     if spec.quant == "fp8" and k % 128 == 0:      # activations are quantised per 128-wide K group
         w = nn.Parameter(torch.zeros(n, k, dtype=torch.float8_e4m3fn, device=device), requires_grad=False)
         s = nn.Parameter(torch.ones((n + 127) // 128, (k + 127) // 128, dtype=torch.float32, device=device),
@@ -118,13 +142,24 @@ def _linear_params(n: int, k: int, spec: ModelSpec, device):
 
 
 def _qw(w, s):
-    """Weight handle passed to the linear ops: plain tensor, or (e4m3, scale_inv) for fp8."""
+    """Weight handle passed to the linear ops: plain tensor, (e4m3, scale_inv) for fp8, `Int4Weight` for int4."""
+    if isinstance(s, W4Params):
+        return ref.Int4Weight(w, s.scales, s.zeros, s.group_size, s.in_features)
     return w if s is None else (w, s)
 
 
-def _store_linear(w_param, s_param, w: torch.Tensor):
+def _store_linear(w_param, s_param, w):
     """Copy a (sharded) weight into its parameter; fp8 parameters are block-quantised here
-    (`weight_utils.fp8_block_quant`)."""
+    (`weight_utils.fp8_block_quant`), int4 ones (`weight_utils.W4Tensor`) repacked into the device layout."""
+    if isinstance(w, wu.W4Tensor):
+        packed, scales, zeros = ref.w4a16_pack(w.codes, w.zeros, w.scales)
+        assert packed.shape == w_param.shape and zeros.shape == s_param.zeros.shape, (packed.shape, w_param.shape)
+        w_param.data.copy_(packed)
+        s_param.zeros.data.copy_(zeros)
+        if s_param.scales.dtype != scales.dtype:     # the checkpoint's 16-bit dtype is kept exactly
+            s_param.scales.data = torch.empty_like(s_param.scales, dtype=scales.dtype)
+        s_param.scales.data.copy_(scales)
+        return
     if s_param is None:
         w_param.data.copy_(w)
         return
@@ -196,10 +231,10 @@ class DenseMLP(nn.Module):
         tp = ps.get_tp_size() if shard else 1
         assert intermediate % tp == 0
         self.inter = intermediate // tp
-        fp8 = spec is not None and spec.quant == "fp8"
+        quant = spec is not None and spec.quant is not None
         # fused SiLU-gate epilogue needs the gate/up rows interleaved per 128 (bf16 kernel only)
-        self.fused_act = self.inter % 128 == 0 and not fp8
-        if fp8:
+        self.fused_act = self.inter % 128 == 0 and not quant
+        if quant:
             self.gate_up_w, self.gate_up_ws = _linear_params(2 * self.inter, hidden, spec, device)
             self.down_w, self.down_ws = _linear_params(hidden, self.inter, spec, device)
         else:
@@ -432,7 +467,13 @@ class CausalLM(nn.Module):
             return dev_gens[device]
 
         for name, p in self.named_parameters():
-            if name.endswith("norm_w"):
+            if p.dtype == torch.int32:       # packed int4 codes: uniform in [0, 15]
+                p.data.view(torch.uint8).random_(0, 256, generator=dev_gen(p.device) if p.is_cuda else g)
+            elif name.endswith("_ws.zeros"):
+                p.data.fill_(8)
+            elif name.endswith("_ws.scales"):
+                p.data.fill_(0.02 / 21.5 ** 0.5)   # std of q - 8 over uniform codes is sqrt(21.5): weight std 0.02
+            elif name.endswith("norm_w"):
                 p.data.fill_(1.0)
             elif p.dim() == 1:
                 p.data.zero_()
@@ -496,16 +537,26 @@ class CausalLM(nn.Module):
                 put(self.lm_head_w, wu.shard_vocab(reader.get(name), tr, tp))
         tick()
 
+    def _linear_weight(self, reader, module: str):
+        """`<module>.weight`, or the module's int4 codes, zeros and scales (`W4Tensor`) for AWQ / GPTQ."""
+        if self.spec.w4 is not None:
+            return reader.get_w4(module, self.spec.w4)
+        return reader.get(module + ".weight")
+
     def _load_attention(self, reader, pre, nm, at: Attention):
         spec, tp, tr, d = self.spec, self.tp_size, self.tp_rank, self.spec.head_dim
         if "qkv_fused" in nm:  # ChatGLM: one [ (hq + 2 hkv) * D, H ] tensor
             w = reader.get(pre + nm["qkv_fused"] + ".weight")
             q, k, v = w.split([spec.num_heads * d, spec.num_kv_heads * d, spec.num_kv_heads * d], dim=0)
         else:
-            q = reader.get(pre + nm["q"] + ".weight")
-            k = reader.get(pre + nm["k"] + ".weight")
-            v = reader.get(pre + nm["v"] + ".weight")
-        _store_linear(at.qkv_w, at.qkv_ws, wu.shard_qkv(q, k, v, spec.num_heads, spec.num_kv_heads, d, tr, tp))
+            q, k, v = (self._linear_weight(reader, pre + nm[x]) for x in ("q", "k", "v"))
+        if isinstance(q, wu.W4Tensor):
+            qkv = wu.W4Tensor(*(
+                wu.shard_qkv(getattr(q, f), getattr(k, f), getattr(v, f), spec.num_heads, spec.num_kv_heads, d, tr,
+                             tp) for f in ("codes", "zeros", "scales")))
+        else:
+            qkv = wu.shard_qkv(q, k, v, spec.num_heads, spec.num_kv_heads, d, tr, tp)
+        _store_linear(at.qkv_w, at.qkv_ws, qkv)
         if at.qkv_b is not None:
             if "qkv_fused" in nm:
                 b = reader.get(pre + nm["qkv_fused"] + ".bias")
@@ -513,7 +564,7 @@ class CausalLM(nn.Module):
             else:
                 qb, kb, vb = (reader.get(pre + nm[x] + ".bias") for x in ("q", "k", "v"))
             at.qkv_b.data.copy_(wu.shard_qkv(qb, kb, vb, spec.num_heads, spec.num_kv_heads, d, tr, tp))
-        _store_linear(at.o_w, at.o_ws, wu.shard_cols(reader.get(pre + nm["o"] + ".weight"), tr, tp))
+        _store_linear(at.o_w, at.o_ws, self._shard_cols(self._linear_weight(reader, pre + nm["o"])))
         if at.o_b is not None:
             at.o_b.data.copy_(reader.get(pre + nm["o"] + ".bias"))
         if at.q_norm_w is not None:
@@ -526,7 +577,15 @@ class CausalLM(nn.Module):
             w = reader.get(pre + nm["gate_up_fused"] + ".weight")
             gate, up = w.chunk(2, dim=0)
         else:
-            gate = reader.get(pre + nm["gate"] + ".weight")
-            up = reader.get(pre + nm["up"] + ".weight")
-        mlp.set_gate_up(wu.shard_gate_up(gate, up, tr, tp))
-        _store_linear(mlp.down_w, mlp.down_ws, wu.shard_cols(reader.get(pre + nm["down"] + ".weight"), tr, tp))
+            gate, up = (self._linear_weight(reader, pre + nm[x]) for x in ("gate", "up"))
+        if isinstance(gate, wu.W4Tensor):
+            mlp.set_gate_up(wu.W4Tensor(*(wu.shard_gate_up(getattr(gate, f), getattr(up, f), tr, tp)
+                                          for f in ("codes", "zeros", "scales"))))
+        else:
+            mlp.set_gate_up(wu.shard_gate_up(gate, up, tr, tp))
+        _store_linear(mlp.down_w, mlp.down_ws, self._shard_cols(self._linear_weight(reader, pre + nm["down"])))
+
+    def _shard_cols(self, w):
+        if isinstance(w, wu.W4Tensor):
+            return wu.shard_cols_w4(w, self.tp_rank, self.tp_size)
+        return wu.shard_cols(w, self.tp_rank, self.tp_size)

@@ -59,6 +59,10 @@ PRESETS = {
                                 "weight_block_size": [128, 128]},
     },
 }
+# 4-bit AWQ builds of the public shapes (group 128, fp16 scales); with dummy weights they need no files
+_AWQ = {"quant_method": "awq", "bits": 4, "group_size": 128, "zero_point": True, "version": "gemm"}
+PRESETS["qwen3-8b-awq"] = dict(PRESETS["qwen3-8b"], torch_dtype="float16", quantization_config=dict(_AWQ))
+PRESETS["llama-3-70b-awq"] = dict(PRESETS["llama-3-70b"], torch_dtype="float16", quantization_config=dict(_AWQ))
 
 
 def tiny(arch: str = "Qwen3ForCausalLM", **over):

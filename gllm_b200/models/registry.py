@@ -12,6 +12,7 @@ from typing import Callable, Dict
 
 import torch
 
+from gllm_b200.models import weight_utils as wu
 from gllm_b200.models.decoder import CausalLM, ModelSpec, MoESpec
 
 _DTYPES = {"bfloat16": torch.bfloat16, "float16": torch.float16, "float32": torch.float32,
@@ -59,6 +60,11 @@ def _base_spec(cfg: HFConfig, arch: str, **kw) -> ModelSpec:
     qc = cfg.get("quantization_config") or {}
     if qc.get("quant_method") == "fp8" and list(qc.get("weight_block_size") or []) == [128, 128]:
         spec.quant = "fp8"
+    spec.w4 = wu.w4_config(qc)
+    if spec.w4 is not None:
+        spec.quant = spec.w4.method
+        if spec.dtype == torch.float16:    # every kernel here is bf16: fp16 tensors are rounded to bf16 once, at load
+            spec.dtype = torch.bfloat16
     for k, v in kw.items():
         setattr(spec, k, v)
     return spec
@@ -183,4 +189,7 @@ def build_model(cfg: HFConfig, device):
     arch = cfg["architectures"][0]
     if arch not in ARCHITECTURES:
         raise ValueError(f"unsupported architecture {arch}; supported: {sorted(ARCHITECTURES)}")
+    if wu.w4_config(cfg.get("quantization_config") or {}) is not None and arch not in wu.W4_ARCHITECTURES:
+        raise ValueError(f"4-bit AWQ / GPTQ weights are not supported for {arch} (supported: "
+                         f"{', '.join(wu.W4_ARCHITECTURES)})")
     return ARCHITECTURES[arch](cfg, device)

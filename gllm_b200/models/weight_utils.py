@@ -7,6 +7,7 @@ from __future__ import annotations
 import glob
 import json
 import os
+from dataclasses import dataclass
 from typing import Dict, List, Optional
 
 import torch
@@ -94,6 +95,95 @@ def fp8_block_quant(w: torch.Tensor):
     sc = (blk.abs().amax(dim=(1, 3)) / 448.0).clamp_min(1e-12)
     q = (blk / sc.view(nb, 1, kb, 1)).view(nb * 128, kb * 128)[:n, :k].to(torch.float8_e4m3fn)
     return q, sc
+
+
+# ------------------------------------------------------------------------------------------------
+# 4-bit AWQ / GPTQ checkpoints
+# ------------------------------------------------------------------------------------------------
+W4_MODULES = ("q_proj", "k_proj", "v_proj", "o_proj", "gate_proj", "up_proj", "down_proj")
+W4_ARCHITECTURES = ("LlamaForCausalLM", "MistralForCausalLM", "Qwen2ForCausalLM", "Qwen3ForCausalLM")
+AWQ_ORDER = (0, 2, 4, 6, 1, 3, 5, 7)   # AWQ: nibble i of a word holds column 8 c + AWQ_ORDER[i]
+
+
+@dataclass
+class W4Config:
+    """A validated AWQ / GPTQ `quantization_config`: 4-bit codes, `group_size` input columns per scale (-1: the whole
+    unsharded K), and `zero_offset` added to the stored zero points (1 for GPTQ v1 checkpoints)."""
+    method: str
+    group_size: int
+    zero_offset: int = 0
+
+
+def w4_config(qc: dict) -> Optional[W4Config]:
+    """Parse `quantization_config`: None for an unquantised or fp8 checkpoint, a `W4Config` for a supported AWQ /
+    GPTQ one; anything else raises ValueError naming the cause."""
+    method = str(qc.get("quant_method", "")).lower() if qc else ""
+    if method in ("", "fp8"):
+        return None
+    if method not in ("awq", "gptq"):
+        raise ValueError(f"quantization method {method!r} is not supported (supported: fp8, awq, gptq)")
+    bits = qc.get("bits", qc.get("w_bit", 4))
+    if bits != 4:
+        raise ValueError(f"{method}: bits={bits} is not supported (only 4-bit weights)")
+    g = qc.get("group_size", qc.get("q_group_size", 128))
+    if g not in (32, 64, 128, -1):
+        raise ValueError(f"{method}: group_size={g} is not supported (32, 64, 128 or -1)")
+    skip = [m for m in (qc.get("modules_to_not_convert") or []) if any(p in m for p in W4_MODULES)]
+    if skip:
+        raise ValueError(f"{method}: modules_to_not_convert names quantised projections {skip}")
+    if method == "awq":
+        version = str(qc.get("version", "gemm")).lower()
+        if version != "gemm":
+            raise ValueError(f"awq: version={version!r} is not supported (only 'gemm')")
+        if not qc.get("zero_point", True):
+            raise ValueError("awq: zero_point=false is not supported")
+        return W4Config("awq", g)
+    if qc.get("desc_act", False):
+        raise ValueError("gptq: desc_act=true (act-order) is not supported")
+    fmt = qc.get("checkpoint_format", "gptq")
+    if fmt not in ("gptq", "gptq_v2"):
+        raise ValueError(f"gptq: checkpoint_format={fmt!r} is not supported ('gptq' or 'gptq_v2')")
+    return W4Config("gptq", g, 1 if fmt == "gptq" else 0)
+
+
+@dataclass
+class W4Tensor:
+    """One quantised linear in checkpoint orientation, whatever the format: codes uint8 [N, K], zeros uint8 [N, G]
+    (with the format's offset applied), scales fp16/bf16 [N, G]."""
+    codes: torch.Tensor
+    zeros: torch.Tensor
+    scales: torch.Tensor
+
+
+def _nibbles(words: torch.Tensor) -> torch.Tensor:
+    """int32 [..., W] -> uint8 [..., W, 8]: nibble i of each word at index i."""
+    w = words.to(torch.int64) & 0xFFFFFFFF
+    return ((w.unsqueeze(-1) >> (4 * torch.arange(8))) & 0xF).to(torch.uint8)
+
+
+def unpack_awq(packed: torch.Tensor) -> torch.Tensor:
+    """AWQ int32 [R, C/8] packed along columns -> uint8 [R, C]."""
+    nib = _nibbles(packed)
+    inv = torch.tensor([AWQ_ORDER.index(j) for j in range(8)])
+    return nib[..., inv].reshape(packed.shape[0], -1)
+
+
+def unpack_gptq_rows(packed: torch.Tensor) -> torch.Tensor:
+    """GPTQ qweight int32 [K/8, N] packed along rows -> uint8 [K, N]."""
+    return _nibbles(packed).permute(0, 2, 1).reshape(-1, packed.shape[1])
+
+
+def unpack_gptq_cols(packed: torch.Tensor) -> torch.Tensor:
+    """GPTQ qzeros int32 [G, N/8] packed along columns -> uint8 [G, N]."""
+    return _nibbles(packed).reshape(packed.shape[0], -1)
+
+
+def shard_cols_w4(w: W4Tensor, rank: int, size: int) -> W4Tensor:
+    """Row-parallel shard of a quantised linear: this rank's K columns and their groups (with one group over the
+    whole K, every rank keeps its zeros and scales)."""
+    one = w.zeros.shape[1] == 1 and w.codes.shape[1] > 1
+    return W4Tensor(shard_cols(w.codes, rank, size), w.zeros if one else shard_cols(w.zeros, rank, size),
+                    w.scales if one else shard_cols(w.scales, rank, size))
 
 
 # ------------------------------------------------------------------------------------------------
@@ -191,6 +281,30 @@ class CheckpointReader:
     def get_fp8(self, name: str):
         """(e4m3 weight, fp32 scale_inv [ceil(N/128), ceil(K/128)])"""
         return self.get_raw(name), self.get_raw(name + "_scale_inv").float()
+
+    def get_w4(self, module: str, cfg: W4Config) -> W4Tensor:
+        """`<module>.qweight / .qzeros / .scales (/ .g_idx)` of an AWQ or GPTQ checkpoint -> `W4Tensor`."""
+        qw, qz = self.get_raw(module + ".qweight"), self.get_raw(module + ".qzeros")
+        scales = self.get_raw(module + ".scales")
+        if cfg.method == "awq":
+            codes = unpack_awq(qw).t()
+            zeros = unpack_awq(qz)
+        else:
+            codes = unpack_gptq_rows(qw).t()
+            zeros = unpack_gptq_cols(qz).to(torch.int32) + cfg.zero_offset
+            k = codes.shape[1]
+            if self.has(module + ".g_idx"):
+                g_idx = self.get_raw(module + ".g_idx").to(torch.int64)
+                want = torch.arange(k) // cfg.group_size if cfg.group_size > 0 else torch.zeros(k, dtype=torch.int64)
+                if not torch.equal(g_idx, want):
+                    raise ValueError(f"{module}: g_idx is not k // group_size (act-order GPTQ is not supported)")
+        n, k = codes.shape
+        groups = 1 if cfg.group_size == -1 else k // cfg.group_size
+        if scales.shape != (groups, n) or zeros.shape != (groups, n) or scales.dtype not in (torch.float16,
+                                                                                              torch.bfloat16):
+            raise ValueError(f"{module}: scales {tuple(scales.shape)} {scales.dtype} / zeros {tuple(zeros.shape)} do "
+                             f"not match {cfg.method} codes [{n}, {k}] with group_size {cfg.group_size}")
+        return W4Tensor(codes.contiguous(), zeros.t().to(torch.uint8).contiguous(), scales.t().contiguous())
 
     def get_rows(self, name: str, start: int, end: int) -> torch.Tensor:
         key = self.resolve(name)

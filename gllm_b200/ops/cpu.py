@@ -12,6 +12,7 @@ import torch
 
 from gllm_b200.ops import ref
 from gllm_b200.ops.lib import GemmComm
+from gllm_b200.ops.ref import Int4Weight
 from gllm_b200.ops.ref import (grouped_topk, kv_copy_pages, logprobs_final,  # noqa: F401  (sm100 signatures)
                                logprobs_shard, prompt_logprobs_shard, rope_kv_write, topk_softmax)
 from gllm_b200.parallel import state as ps
@@ -25,9 +26,17 @@ def _into(out: Optional[torch.Tensor], y: torch.Tensor) -> torch.Tensor:
 def linear(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None,
            out: Optional[torch.Tensor] = None, comm: Optional[GemmComm] = None, epi: int = 0) -> torch.Tensor:
     assert comm is None and epi == 0, "GEMM epilogues over peer memory are sm_90a only"
+    if isinstance(w, Int4Weight):
+        return linear_w4a16(x, w, bias, out=out)
     if isinstance(w, tuple):
         return linear_fp8_block(x, w[0], w[1], bias, out=out)
     return _into(out, ref.linear(x, w, bias))
+
+
+def linear_w4a16(x: torch.Tensor, w: Int4Weight, bias: Optional[torch.Tensor] = None,
+                 out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The device layout unpacked and de-quantised to x's dtype (`ref.w4a16_dequant`), then `ref.linear`."""
+    return _into(out, ref.linear_w4a16(x, w, bias))
 
 
 def linear_silu_mul(x: torch.Tensor, w_interleaved: torch.Tensor, out: Optional[torch.Tensor] = None,

@@ -56,6 +56,7 @@ def _declare(lib):
     sig("gllm_gemm_tune", [I, I])
     sig("gllm_gemm_bf16_batched", [P, L, L, P, P, L, L, I, I, I, I, P])
     sig("gllm_gemm_smallm", [P, L, P, L, P, L, I, I, I, P, I, I, P, L, P, P])
+    sig("gllm_gemm_w4a16", [P, L, P, P, P, I, I, P, L, I, I, I, P, I, P, L, P, L, P])
     sig("gllm_rmsnorm", [P, P, P, P, P, I, I, L, F, P])
     sig("gllm_silu_and_mul", [P, P, I, I, L, P])
     sig("gllm_embedding", [P, P, P, I, I, I, I, P])

@@ -684,3 +684,92 @@ def lora_expand_silu_mul(pre: torch.Tensor, u: torch.Tensor, B: torch.Tensor, sl
         d[rr] = torch.where(gate_col, u[rr, :r] @ B[s].float().t(), u[rr, r:2 * r] @ B[s].float().t())
     y = (pre.float() + d).reshape(t, two_i // (2 * block), 2, block)
     return (F.silu(y[:, :, 0]) * y[:, :, 1]).to(pre.dtype).reshape(t, two_i // 2)
+
+
+# ----------------------------------------------------------------------------------------------
+# W4A16: int4 weights with 16-bit group scales and uint8 zero points (AWQ / GPTQ checkpoints)
+# ----------------------------------------------------------------------------------------------
+class Int4Weight:
+    """Weight handle of a W4A16 linear, in the device layout of csrc/gemm/gemm_w4a16.cu (the same on every device):
+    `packed` int32 [round_up(N, 16), round_up(K, 128) / 8], `scales` fp16/bf16 [G, N], `zeros` uint8
+    [G, round_up(N, 16)], with G = ceil(K / group_size). `group_size` >= K means one group. Not a tuple: the linear
+    ops send tuples to the fp8 block GEMM."""
+    __slots__ = ("packed", "scales", "zeros", "group_size", "in_features")
+
+    def __init__(self, packed, scales, zeros, group_size: int, in_features: int):
+        self.packed, self.scales, self.zeros = packed, scales, zeros
+        self.group_size, self.in_features = int(group_size), int(in_features)
+
+    @property
+    def out_features(self) -> int:
+        return self.scales.shape[1]
+
+
+W4_BLOCK_K = 128
+
+
+def _w4_fragment_index():
+    """[256 words, 8 nibbles] -> (row, k) index (row * 128 + k) inside one 16-row x 128-k block of the device layout:
+    word p = 128 h + 4 lane + j holds lane's m64k16 A fragment of k-step 4 h + j; nibble e is fragment element e, at
+    row lane / 4 (+ 8 for e = 2, 3, 6, 7) and column 2 (lane % 4) + e % 2 (+ 8 for e >= 4)."""
+    p = torch.arange(256).view(256, 1)
+    e = torch.arange(8).view(1, 8)
+    h, lane, j = p // 128, (p // 4) % 32, p % 4
+    row = lane // 4 + 8 * ((e // 2) % 2)
+    col = 16 * (4 * h + j) + 2 * (lane % 4) + e % 2 + 8 * (e // 4)
+    return row * W4_BLOCK_K + col
+
+
+_W4_IDX = _w4_fragment_index()
+
+
+def w4a16_pack(codes: torch.Tensor, zeros: torch.Tensor, scales: torch.Tensor):
+    """Checkpoint orientation -> device layout. codes uint8 [N, K] in [0, 15], zeros uint8 [N, G], scales 16-bit
+    [N, G] -> (packed, scales [G, N], zeros [G, Np]); see `Int4Weight`."""
+    n, k = codes.shape
+    np_, kp = -(-n // 16) * 16, -(-k // W4_BLOCK_K) * W4_BLOCK_K
+    c = torch.zeros(np_, kp, dtype=torch.int64)
+    c[:n, :k] = codes.to(torch.int64)
+    blocks = c.view(np_ // 16, 16, kp // W4_BLOCK_K, W4_BLOCK_K).permute(0, 2, 1, 3).reshape(
+        np_ // 16, kp // W4_BLOCK_K, 16 * W4_BLOCK_K)
+    nib = blocks[:, :, _W4_IDX.view(-1)].view(np_ // 16, kp // W4_BLOCK_K, 256, 8)
+    words = (nib << (4 * torch.arange(8))).sum(-1)
+    words = torch.where(words >= 2 ** 31, words - 2 ** 32, words).to(torch.int32)
+    packed = words.view(np_ // 16, kp // W4_BLOCK_K, 16, 16).permute(0, 2, 1, 3).reshape(np_, kp // 8)
+    z = torch.zeros(zeros.shape[1], np_, dtype=torch.uint8)
+    z[:, :n] = zeros.t()
+    return packed.contiguous(), scales.t().contiguous(), z
+
+
+def w4a16_unpack(w: Int4Weight):
+    """Device layout -> checkpoint orientation: (codes uint8 [N, K], zeros uint8 [N, G], scales [N, G])."""
+    packed = w.packed.cpu()
+    np_, kw = packed.shape
+    kp = kw * 8
+    words = packed.view(np_ // 16, 16, kp // W4_BLOCK_K, 16).permute(0, 2, 1, 3).reshape(
+        np_ // 16, kp // W4_BLOCK_K, 256, 1).to(torch.int64) & 0xFFFFFFFF
+    nib = (words >> (4 * torch.arange(8))) & 0xF
+    blocks = torch.empty(np_ // 16, kp // W4_BLOCK_K, 16 * W4_BLOCK_K, dtype=torch.int64)
+    blocks[:, :, _W4_IDX.view(-1)] = nib.view(np_ // 16, kp // W4_BLOCK_K, 2048)
+    codes = blocks.view(np_ // 16, kp // W4_BLOCK_K, 16, W4_BLOCK_K).permute(0, 2, 1, 3).reshape(np_, kp)
+    n, k = w.out_features, w.in_features
+    return (codes[:n, :k].to(torch.uint8), w.zeros.cpu()[:, :n].t().contiguous(),
+            w.scales.cpu().t().contiguous())
+
+
+def w4a16_dequant(codes: torch.Tensor, zeros: torch.Tensor, scales: torch.Tensor, group_size: int,
+                  dtype: torch.dtype) -> torch.Tensor:
+    """W [N, K] = dtype( fp32(s) · (q − z) ): exact in fp32 (a 16-bit scale has at most 11 significant bits and
+    |q − z| <= 16), rounded once. Column k uses group k // group_size (one group if group_size >= K)."""
+    k = codes.shape[1]
+    gi = torch.arange(k) // group_size if group_size < k else torch.zeros(k, dtype=torch.long)
+    q = codes.to(torch.float32)
+    z = zeros.to(torch.float32)[:, gi]
+    s = scales.to(torch.float32)[:, gi]
+    return (s * (q - z)).to(dtype)
+
+
+def linear_w4a16(x: torch.Tensor, w: Int4Weight, bias: Optional[torch.Tensor] = None) -> torch.Tensor:
+    codes, zeros, scales = w4a16_unpack(w)
+    wd = w4a16_dequant(codes, zeros, scales, w.group_size, x.dtype).to(x.device)
+    return linear(x, wd, bias)

@@ -13,6 +13,7 @@ import torch
 
 from gllm_b200.ops import lib as _lib
 from gllm_b200.ops.lib import GemmComm, check, stream_ptr
+from gllm_b200.ops.ref import Int4Weight
 
 _BF16 = torch.bfloat16
 NUM_SMS = 132   # H100 SXM
@@ -70,7 +71,10 @@ def _linear_smallm(x, w, bias, out, silu: bool):
 
 def linear(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None,
            out: Optional[torch.Tensor] = None, comm: Optional[GemmComm] = None, epi: int = 0) -> torch.Tensor:
-    """y = x @ w.T (+ bias). x [M, K] (row stride arbitrary, unit inner stride), w [N, K] or (e4m3, scale_inv)."""
+    """y = x @ w.T (+ bias). x [M, K] (row stride arbitrary, unit inner stride), w [N, K], (e4m3, scale_inv) or an
+    `Int4Weight`."""
+    if isinstance(w, Int4Weight):
+        return linear_w4a16(x, w, bias, out=out)
     if isinstance(w, tuple):
         return linear_fp8_block(x, w[0], w[1], bias, out=out)
     assert x.dtype == _BF16 and w.dtype == _BF16, (x.dtype, w.dtype)
@@ -118,6 +122,37 @@ def linear_silu_mul(x: torch.Tensor, w_interleaved: torch.Tensor, out: Optional[
                           ctypes.byref(comm) if comm is not None else None, _p(ws), ws.numel() * 4, _p(tcnt),
                           _SPLITK_MAX_TILES, stream_ptr())
     check(rc, "gemm_bf16(silu)")
+    _count()
+    return out
+
+
+_W4_FORCE_SPLIT = int(os.environ.get("GLLM_W4_SPLIT", "0"))
+
+
+def linear_w4a16(x: torch.Tensor, w: Int4Weight, bias: Optional[torch.Tensor] = None,
+                 out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """y = x @ W.T (+ bias) with W the de-quantised int4 weight of `w` (csrc/gemm/gemm_w4a16.cu), x bf16 [M, K] (row
+    stride a multiple of 8, unit inner stride). Split-K partials use the small-M workspace (allocated before graph
+    capture) and are reduced in a fixed order."""
+    assert isinstance(w, Int4Weight) and w.packed.dtype == torch.int32 and w.zeros.dtype == torch.uint8
+    assert w.scales.dtype in (torch.float16, _BF16) and w.packed.is_contiguous() and w.scales.is_contiguous()
+    assert x.dtype == _BF16 and x.dim() == 2 and x.stride(1) == 1 and x.shape[1] == w.in_features, (x.shape,
+                                                                                                   w.in_features)
+    assert x.data_ptr() % 16 == 0 and x.stride(0) % 8 == 0, "TMA needs 16-byte aligned rows"
+    m, k = x.shape
+    n = w.out_features
+    if out is None:
+        out = torch.empty(m, n, dtype=_BF16, device=x.device)
+    else:
+        assert out.shape == (m, n) and out.stride(1) == 1 and out.dtype == _BF16
+    if m == 0:
+        return out
+    ws, _, tcnt = _smallm_workspace(x.device)
+    L = _lib.load()
+    rc = L.gllm_gemm_w4a16(_p(x), x.stride(0), _p(w.packed), _p(w.scales), _p(w.zeros),
+                           1 if w.scales.dtype == _BF16 else 0, w.group_size, _p(out), out.stride(0), m, n, k,
+                           _p(bias), _W4_FORCE_SPLIT, _p(ws), ws.numel(), _p(tcnt), tcnt.numel(), stream_ptr())
+    check(rc, "gemm_w4a16")
     _count()
     return out
 
