@@ -16,7 +16,6 @@ from gllm_b200.ops import lib as _lib, ref, sm100  # noqa: E402
 
 def main():
     L = _lib.load()
-    L.gllm_gemm_tune.argtypes = [_lib.c_int, _lib.c_int]
     H, I, QKV = 4096, 12288, 6144
     for m in (64, 128, 256, 384, 512):
         for n, k, name, silu in ((QKV, H, "qkv", False), (H, H, "o", False), (2 * I, H, "gate_up", True),

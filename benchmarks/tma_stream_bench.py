@@ -1,5 +1,4 @@
 """HBM -> SMEM streaming micro-benchmark (TMA box shapes / bulk copies / LDG). Prints GB/s."""
-import ctypes
 import os
 import sys
 
@@ -9,9 +8,6 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from gllm_b200.ops import lib as _lib  # noqa: E402
 
 L = _lib.load()
-P, I, LL = ctypes.c_void_p, ctypes.c_int, ctypes.c_int64
-L.gllm_bench_tma_stream.argtypes = [P, LL, LL, LL, I, I, I, I, I, P, P]
-L.gllm_bench_tma_stream.restype = I
 rows, cols = 24576, 4096  # 201 MB, like the gate/up weight
 w = torch.randn(rows, cols, device="cuda").bfloat16()
 sink = torch.zeros(1, dtype=torch.int64, device="cuda")

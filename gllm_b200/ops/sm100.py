@@ -5,35 +5,19 @@ CUDA stream. No fallback: if the library is missing on a GPU box this raises.
 """
 from __future__ import annotations
 
-import ctypes
 import os
 from typing import Optional
 
 import torch
 
 from gllm_b200.ops import lib as _lib
-from gllm_b200.ops.lib import GemmComm, check, stream_ptr
+from gllm_b200.ops.lib import GemmComm, _p, check, launch, launches, stream_ptr  # noqa: F401 (launches: bench.py)
 from gllm_b200.ops.ref import Int4Weight
+# the MoE front-ends, so that a model module sees one table
+from gllm_b200.ops.sm100_moe import fused_experts, fused_experts_fp8, grouped_topk, topk_softmax  # noqa: F401
 
 _BF16 = torch.bfloat16
 NUM_SMS = 132   # H100 SXM
-
-
-def _p(t: Optional[torch.Tensor]):
-    return None if t is None else ctypes.c_void_p(t.data_ptr())
-
-
-_launch_count = 0
-
-
-def launches() -> int:
-    """Number of kernel launches issued through this module (bench.py `gpu_launches`)."""
-    return _launch_count
-
-
-def _count(n=1):
-    global _launch_count
-    _launch_count += n
 
 
 # ----------------------------------------------------------------------------------------------
@@ -61,11 +45,8 @@ def _linear_smallm(x, w, bias, out, silu: bool):
     m, k = x.shape
     n = w.shape[0]
     ws, cnt, _ = _smallm_workspace(x.device)
-    L = _lib.load()
-    rc = L.gllm_gemm_smallm(_p(x), x.stride(0), _p(w), w.stride(0), _p(out), out.stride(0), m, n, k, _p(bias),
-                            1 if silu else 0, _FORCE_SPLIT, _p(ws), ws.numel(), _p(cnt), stream_ptr())
-    check(rc, "gemm_smallm")
-    _count()
+    launch("gllm_gemm_smallm", _p(x), x.stride(0), _p(w), w.stride(0), _p(out), out.stride(0), m, n, k, _p(bias),
+           1 if silu else 0, _FORCE_SPLIT, _p(ws), ws.numel(), _p(cnt))
     return out
 
 
@@ -91,13 +72,9 @@ def linear(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None
         return out
     if comm is None and epi == 0 and _FORCE_BN == 0 and (m <= _SMALLM_MAX or (m <= 64 and k >= 8192)):
         return _linear_smallm(x, w, bias, out, False)
-    L = _lib.load()
     ws, _, tcnt = _smallm_workspace(x.device)
-    rc = L.gllm_gemm_bf16(_p(x), x.stride(0), _p(w), w.stride(0), _p(out), out.stride(0), m, n, k, _p(bias),
-                          epi, _FORCE_BN, ctypes.byref(comm) if comm is not None else None, _p(ws),
-                          ws.numel() * 4, _p(tcnt), _SPLITK_MAX_TILES, stream_ptr())
-    check(rc, "gemm_bf16")
-    _count()
+    launch("gllm_gemm_bf16", _p(x), x.stride(0), _p(w), w.stride(0), _p(out), out.stride(0), m, n, k, _p(bias), epi,
+           _FORCE_BN, comm, _p(ws), ws.numel() * 4, _p(tcnt), _SPLITK_MAX_TILES)
     return out
 
 
@@ -115,14 +92,9 @@ def linear_silu_mul(x: torch.Tensor, w_interleaved: torch.Tensor, out: Optional[
         return out
     if m <= _SMALLM_MAX and _FORCE_BN == 0 and comm is None:
         return _linear_smallm(x, w_interleaved, None, out, True)
-    L = _lib.load()
     ws, _, tcnt = _smallm_workspace(x.device)
-    rc = L.gllm_gemm_bf16(_p(x), x.stride(0), _p(w_interleaved), w_interleaved.stride(0), _p(out),
-                          out.stride(0), m, n, k, None, 1, 256,
-                          ctypes.byref(comm) if comm is not None else None, _p(ws), ws.numel() * 4, _p(tcnt),
-                          _SPLITK_MAX_TILES, stream_ptr())
-    check(rc, "gemm_bf16(silu)")
-    _count()
+    launch("gllm_gemm_bf16", _p(x), x.stride(0), _p(w_interleaved), w_interleaved.stride(0), _p(out), out.stride(0),
+           m, n, k, None, 1, 256, comm, _p(ws), ws.numel() * 4, _p(tcnt), _SPLITK_MAX_TILES)
     return out
 
 
@@ -148,12 +120,9 @@ def linear_w4a16(x: torch.Tensor, w: Int4Weight, bias: Optional[torch.Tensor] = 
     if m == 0:
         return out
     ws, _, tcnt = _smallm_workspace(x.device)
-    L = _lib.load()
-    rc = L.gllm_gemm_w4a16(_p(x), x.stride(0), _p(w.packed), _p(w.scales), _p(w.zeros),
-                           1 if w.scales.dtype == _BF16 else 0, w.group_size, _p(out), out.stride(0), m, n, k,
-                           _p(bias), _W4_FORCE_SPLIT, _p(ws), ws.numel(), _p(tcnt), tcnt.numel(), stream_ptr())
-    check(rc, "gemm_w4a16")
-    _count()
+    launch("gllm_gemm_w4a16", _p(x), x.stride(0), _p(w.packed), _p(w.scales), _p(w.zeros),
+           1 if w.scales.dtype == _BF16 else 0, w.group_size, _p(out), out.stride(0), m, n, k, _p(bias),
+           _W4_FORCE_SPLIT, _p(ws), ws.numel(), _p(tcnt), tcnt.numel())
     return out
 
 
@@ -170,11 +139,7 @@ def rmsnorm(x: torch.Tensor, w: torch.Tensor, eps: float, residual: Optional[tor
         assert residual.is_contiguous()
         if residual_out is None:
             residual_out = residual  # in place, like the reference's fused_add_rms_norm
-    L = _lib.load()
-    rc = L.gllm_rmsnorm(_p(x), _p(residual), _p(w), _p(out), _p(residual_out), t, h, x.stride(0), float(eps),
-                        stream_ptr())
-    check(rc, "rmsnorm")
-    _count()
+    launch("gllm_rmsnorm", _p(x), _p(residual), _p(w), _p(out), _p(residual_out), t, h, x.stride(0), float(eps))
     return out, residual_out
 
 
@@ -184,9 +149,7 @@ def silu_and_mul(x: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.T
     i = two_i // 2
     if out is None:
         out = torch.empty(t, i, dtype=_BF16, device=x.device)
-    L = _lib.load()
-    check(L.gllm_silu_and_mul(_p(x), _p(out), t, i, x.stride(0), stream_ptr()), "silu_and_mul")
-    _count()
+    launch("gllm_silu_and_mul", _p(x), _p(out), t, i, x.stride(0))
     return out
 
 
@@ -198,9 +161,7 @@ def embedding(ids: torch.Tensor, table: torch.Tensor, vocab_start: int = 0, voca
     vocab_end = vocab_start + table.shape[0] if vocab_end is None else vocab_end
     if out is None:
         out = torch.empty(t, h, dtype=_BF16, device=table.device)
-    L = _lib.load()
-    check(L.gllm_embedding(_p(ids), _p(table), _p(out), t, h, vocab_start, vocab_end, stream_ptr()), "embedding")
-    _count()
+    launch("gllm_embedding", _p(ids), _p(table), _p(out), t, h, vocab_start, vocab_end)
     return out
 
 
@@ -209,9 +170,7 @@ def gather_rows(src: torch.Tensor, idx: torch.Tensor, out: Optional[torch.Tensor
     n, h = idx.shape[0], src.shape[1]
     if out is None:
         out = torch.empty(n, h, dtype=_BF16, device=src.device)
-    L = _lib.load()
-    check(L.gllm_gather_rows(_p(src), _p(idx), _p(out), n, h, stream_ptr()), "gather_rows")
-    _count()
+    launch("gllm_gather_rows", _p(src), _p(idx), _p(out), n, h)
     return out
 
 
@@ -245,15 +204,11 @@ def rope_kv_write(q: torch.Tensor, k: torch.Tensor, v: Optional[torch.Tensor], p
         pos_stride = positions.stride(0)
     elif positions.dim() == 2:
         positions = positions[0]
-    L = _lib.load()
-    rc = L.gllm_rope_kv_write(
-        _p(q), q.stride(0), q.stride(1), hq, _p(k), k.stride(0), k.stride(1), hkv,
-        _p(v), v.stride(0) if v is not None else 0, v.stride(1) if v is not None else 0,
-        _p(q_norm_w), _p(k_norm_w), _p(cos_sin), d, rot_dim if cos_sin is not None else 0, 1 if neox else 0, t,
-        _p(positions), _p(slots), float(eps), _p(k_cache), _p(v_cache), sec0, sec1, page_size, pos_stride,
-        stream_ptr())
-    check(rc, "rope_kv_write")
-    _count()
+    launch("gllm_rope_kv_write",
+           _p(q), q.stride(0), q.stride(1), hq, _p(k), k.stride(0), k.stride(1), hkv,
+           _p(v), v.stride(0) if v is not None else 0, v.stride(1) if v is not None else 0,
+           _p(q_norm_w), _p(k_norm_w), _p(cos_sin), d, rot_dim if cos_sin is not None else 0, 1 if neox else 0, t,
+           _p(positions), _p(slots), float(eps), _p(k_cache), _p(v_cache), sec0, sec1, page_size, pos_stride)
 
 
 # ----------------------------------------------------------------------------------------------
@@ -327,8 +282,6 @@ def paged_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tenso
     assert block_table.dtype == torch.int32 and seq_lens.dtype == torch.int32
     if out is None:
         out = torch.empty(t, hq * d, dtype=_BF16, device=q.device)
-    L = _lib.load()
-    st = stream_ptr()
     max_blocks = block_table.shape[1]
     if num_decode_seqs > 0:
         if splits is None:
@@ -340,28 +293,24 @@ def paged_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tenso
             part_lse = _workspace(q.device, num_decode_seqs * hq * splits, "part_lse")
             if _FUSED_MERGE:   # last split CTA merges in-kernel; measured 4 % slower end to end than the
                 split_cnt = _split_counters(q.device, num_decode_seqs * hq)   # PDL-launched merge kernel
-        rc = L.gllm_attn_decode(_p(q), q.stride(0), _p(out), _p(k_cache), _p(v_cache), pages, _p(block_table),
-                                _p(seq_lens), _p(part_o), _p(part_lse), num_decode_seqs, 0, max_blocks, hq, hkv, d,
-                                page_size, splits, float(scale), _p(split_cnt), st)
-        check(rc, "attn_decode")
-        _count(1 if (splits == 1 or split_cnt is not None) else 2)
+        launch("gllm_attn_decode", _p(q), q.stride(0), _p(out), _p(k_cache), _p(v_cache), pages, _p(block_table),
+               _p(seq_lens), _p(part_o), _p(part_lse), num_decode_seqs, 0, max_blocks, hq, hkv, d, page_size, splits,
+               float(scale), _p(split_cnt), n=1 if (splits == 1 or split_cnt is not None) else 2)
     n_prefill = num_seqs - num_decode_seqs
     if n_prefill > 0:
         assert query_start_loc.dtype == torch.int32
-        rc = 2
         if ATTN_TC:
-            rc = L.gllm_attn_prefill_tc(_p(q), q.stride(0), _p(out), _p(k_cache), _p(v_cache), pages, _p(block_table),
-                                        _p(seq_lens), _p(query_start_loc), n_prefill, num_decode_seqs, max_q_len,
-                                        max_blocks, hq, hkv, d, page_size, float(scale), ATTN_TC_KV, st)
+            rc = _lib.load().gllm_attn_prefill_tc(
+                _p(q), q.stride(0), _p(out), _p(k_cache), _p(v_cache), pages, _p(block_table), _p(seq_lens),
+                _p(query_start_loc), n_prefill, num_decode_seqs, max_q_len, max_blocks, hq, hkv, d, page_size,
+                float(scale), ATTN_TC_KV, stream_ptr())
             if rc != 2:                     # 2 = shape outside the wgmma kernel's envelope -> mma.sync kernel
-                check(rc, "attn_prefill_tc")
-                _count()
+                check(rc, "gllm_attn_prefill_tc")
+                _lib._count()
                 return out
-        rc = L.gllm_attn_prefill(_p(q), q.stride(0), _p(out), _p(k_cache), _p(v_cache), pages, _p(block_table),
-                                 _p(seq_lens), _p(query_start_loc), n_prefill, num_decode_seqs, max_q_len,
-                                 max_blocks, hq, hkv, d, page_size, float(scale), st)
-        check(rc, "attn_prefill")
-        _count()
+        launch("gllm_attn_prefill", _p(q), q.stride(0), _p(out), _p(k_cache), _p(v_cache), pages, _p(block_table),
+               _p(seq_lens), _p(query_start_loc), n_prefill, num_decode_seqs, max_q_len, max_blocks, hq, hkv, d,
+               page_size, float(scale))
     return out
 
 
@@ -375,11 +324,8 @@ def gemm_batched(a: torch.Tensor, w: torch.Tensor, out: torch.Tensor) -> torch.T
     assert w.shape == (b, n, k) and w.is_contiguous() and out.shape == (t, b, n)
     assert a.dtype == _BF16 and w.dtype == _BF16 and out.dtype == _BF16
     assert a.stride(2) == 1 and out.stride(2) == 1
-    L = _lib.load()
-    rc = L.gllm_gemm_bf16_batched(_p(a), a.stride(0), a.stride(1), _p(w), _p(out), out.stride(0), out.stride(1),
-                                  t, b, n, k, stream_ptr())
-    check(rc, "gemm_bf16_batched")
-    _count()
+    launch("gllm_gemm_bf16_batched", _p(a), a.stride(0), a.stride(1), _p(w), _p(out), out.stride(0), out.stride(1),
+           t, b, n, k)
     return out
 
 
@@ -404,14 +350,9 @@ def sample(logits: torch.Tensor, temperature=None, top_k=None, top_p=None, rep_p
     if out is None:
         out = torch.empty(b, dtype=torch.int32, device=logits.device)
     seen_words = seen_bits.shape[1] if seen_bits is not None else 0
-    L = _lib.load()
-    rc = L.gllm_sample(_p(logits), dtype, logits.stride(0), _p(out), b, v, _p(temperature), _p(top_k), _p(top_p),
-                       _p(rep_penalty), _p(seen_bits), seen_words, _p(slot_idx),
-                       ctypes.c_uint64(seed & ((1 << 64) - 1)),
-                       _p(step), _p(out_max), vocab_offset, *_bias_seed_args(bias, bias_slot, seeds, seed_pos),
-                       stream_ptr())
-    check(rc, "sample")
-    _count()
+    launch("gllm_sample", _p(logits), dtype, logits.stride(0), _p(out), b, v, _p(temperature), _p(top_k), _p(top_p),
+           _p(rep_penalty), _p(seen_bits), seen_words, _p(slot_idx), seed & ((1 << 64) - 1), _p(step), _p(out_max),
+           vocab_offset, *_bias_seed_args(bias, bias_slot, seeds, seed_pos))
     return out
 
 
@@ -437,13 +378,9 @@ def vp_candidates(shard: torch.Tensor, valid: int, v_full: int, c: int, temperat
     b = shard.shape[0]
     out = torch.empty(b, 2 * c + 4, dtype=torch.float32, device=shard.device)
     seen_words = seen_bits.shape[1] if seen_bits is not None else 0
-    L = _lib.load()
-    rc = L.gllm_vp_candidates(_p(shard), 0 if shard.dtype == _BF16 else 1, shard.stride(0), _p(out), b, valid, v_full,
-                              c, _p(temperature), _p(top_k), _p(top_p), _p(rep_penalty), _p(seen_bits), seen_words,
-                              _p(slot_idx), ctypes.c_uint64(seed & ((1 << 64) - 1)), _p(step), vocab_offset,
-                              *_bias_seed_args(bias, bias_slot, seeds, seed_pos), stream_ptr())
-    check(rc, "vp_candidates")
-    _count()
+    launch("gllm_vp_candidates", _p(shard), 0 if shard.dtype == _BF16 else 1, shard.stride(0), _p(out), b, valid,
+           v_full, c, _p(temperature), _p(top_k), _p(top_p), _p(rep_penalty), _p(seen_bits), seen_words, _p(slot_idx),
+           seed & ((1 << 64) - 1), _p(step), vocab_offset, *_bias_seed_args(bias, bias_slot, seeds, seed_pos))
     return out
 
 
@@ -454,12 +391,8 @@ def vp_final(gathered: torch.Tensor, c: int, v_full: int, top_k=None, top_p=None
     tp, b, w = gathered.shape
     assert w == 2 * c + 4 and gathered.is_contiguous() and gathered.dtype == torch.float32
     out = torch.empty(b, dtype=torch.int32, device=gathered.device)
-    L = _lib.load()
-    rc = L.gllm_vp_final(_p(gathered), tp, b, c, v_full, _p(top_k), _p(top_p),
-                         ctypes.c_uint64(seed & ((1 << 64) - 1)), _p(step), _p(out),
-                         *_bias_seed_args(None, None, seeds, seed_pos)[3:], stream_ptr())
-    check(rc, "vp_final")
-    _count()
+    launch("gllm_vp_final", _p(gathered), tp, b, c, v_full, _p(top_k), _p(top_p), seed & ((1 << 64) - 1), _p(step),
+           _p(out), *_bias_seed_args(None, None, seeds, seed_pos)[3:])
     return out
 
 
@@ -478,11 +411,8 @@ def logprobs_shard(logits: torch.Tensor, valid: int, n: int, tokens: torch.Tenso
     assert rows is None or (rows.dtype == torch.int32 and rows.is_contiguous())
     e = logits.shape[0] if rows is None else rows.numel()
     out = torch.empty(e, 2 * n + 3, dtype=torch.float32, device=logits.device)
-    L = _lib.load()
-    rc = L.gllm_logprobs_shard(_p(logits), 0 if logits.dtype == _BF16 else 1, logits.stride(0), e, valid, n, _p(rows),
-                               _p(tokens), _p(out), vocab_offset, stream_ptr())
-    check(rc, "logprobs_shard")
-    _count()
+    launch("gllm_logprobs_shard", _p(logits), 0 if logits.dtype == _BF16 else 1, logits.stride(0), e, valid, n,
+           _p(rows), _p(tokens), _p(out), vocab_offset)
     return out
 
 
@@ -498,11 +428,8 @@ def prompt_logprobs_shard(logits: torch.Tensor, valid: int, n: int, targets: tor
     if out is None:
         out = torch.empty(q, 2 * n + 3, dtype=torch.float32, device=logits.device)
     assert out.shape == (q, 2 * n + 3) and out.is_contiguous() and out.dtype == torch.float32
-    L = _lib.load()
-    rc = L.gllm_prompt_logprobs_shard(_p(logits), 0 if logits.dtype == _BF16 else 1, logits.stride(0), q, valid, n,
-                                      _p(targets), _p(out), vocab_offset, stream_ptr())
-    check(rc, "prompt_logprobs_shard")
-    _count()
+    launch("gllm_prompt_logprobs_shard", _p(logits), 0 if logits.dtype == _BF16 else 1, logits.stride(0), q, valid,
+           n, _p(targets), _p(out), vocab_offset)
     return out
 
 
@@ -513,9 +440,7 @@ def logprobs_final(gathered: torch.Tensor, n: int) -> torch.Tensor:
     tp, e, w = gathered.shape
     assert w == 2 * n + 3 and gathered.is_contiguous() and gathered.dtype == torch.float32
     out = torch.empty(e, 1 + 2 * n, dtype=torch.float32, device=gathered.device)
-    L = _lib.load()
-    check(L.gllm_logprobs_final(_p(gathered), tp, e, n, _p(out), stream_ptr()), "logprobs_final")
-    _count()
+    launch("gllm_logprobs_final", _p(gathered), tp, e, n, _p(out))
     return out
 
 
@@ -526,10 +451,8 @@ def bias_account(bias: torch.Tensor, out_seen: torch.Tensor, bias_slot: torch.Te
     e = bias_slot.numel()
     assert tokens.dtype == torch.int32 and tokens.numel() >= e and bias_slot.dtype == torch.int32
     assert freq.dtype == torch.float32 and pres.dtype == torch.float32 and bias.stride(1) == 1
-    L = _lib.load()
-    check(L.gllm_bias_account(_p(bias), bias.stride(0), _p(out_seen), out_seen.shape[1], _p(bias_slot), _p(tokens),
-                              _p(freq), _p(pres), e, stream_ptr()), "bias_account")
-    _count()
+    launch("gllm_bias_account", _p(bias), bias.stride(0), _p(out_seen), out_seen.shape[1], _p(bias_slot), _p(tokens),
+           _p(freq), _p(pres), e)
 
 
 def bias_rebuild(bias: torch.Tensor, out_seen: torch.Tensor, v: int, slots: torch.Tensor, pen: torch.Tensor,
@@ -541,11 +464,8 @@ def bias_rebuild(bias: torch.Tensor, out_seen: torch.Tensor, v: int, slots: torc
     for t, dt in ((slots, torch.int32), (pen, torch.float32), (lb_off, torch.int32), (lb_ids, torch.int32),
                   (lb_vals, torch.float32), (out_off, torch.int32), (out_toks, torch.int32)):
         assert t.dtype == dt and t.is_contiguous()
-    L = _lib.load()
-    check(L.gllm_bias_rebuild(_p(bias), bias.stride(0), _p(out_seen), out_seen.shape[1], v, r, _p(slots), _p(pen),
-                              _p(lb_off), _p(lb_ids), _p(lb_vals), _p(out_off), _p(out_toks), stream_ptr()),
-          "bias_rebuild")
-    _count()
+    launch("gllm_bias_rebuild", _p(bias), bias.stride(0), _p(out_seen), out_seen.shape[1], v, r, _p(slots), _p(pen),
+           _p(lb_off), _p(lb_ids), _p(lb_vals), _p(out_off), _p(out_toks))
 
 
 _kv_bases = {}
@@ -576,18 +496,13 @@ def kv_copy_pages(tensors, pairs, dummy_page: Optional[int] = None):
 def launch_kv_copy_pages(tensors, bases: torch.Tensor, dev_pairs: torch.Tensor):
     """The launch alone: `bases` int64 [len(tensors)] and `dev_pairs` int32 [n, 2] already on the device and checked."""
     t0 = tensors[0]
-    L = _lib.load()
-    check(L.gllm_kv_copy_pages(_p(bases), len(tensors), t0[0].numel() * t0.element_size(), _p(dev_pairs),
-                               dev_pairs.shape[0], stream_ptr()), "kv_copy_pages")
-    _count()
+    launch("gllm_kv_copy_pages", _p(bases), len(tensors), t0[0].numel() * t0.element_size(), _p(dev_pairs),
+           dev_pairs.shape[0])
 
 
 def mark_seen(seen_bits: torch.Tensor, rows: torch.Tensor, tokens: torch.Tensor):
     assert rows.dtype == torch.int32 and tokens.dtype == torch.int32
-    L = _lib.load()
-    check(L.gllm_mark_seen(_p(seen_bits), seen_bits.shape[1], _p(rows), _p(tokens), rows.numel(), stream_ptr()),
-          "mark_seen")
-    _count()
+    launch("gllm_mark_seen", _p(seen_bits), seen_bits.shape[1], _p(rows), _p(tokens), rows.numel())
 
 
 # ----------------------------------------------------------------------------------------------
@@ -599,9 +514,7 @@ def fp8_quant_group(x: torch.Tensor):
     m, k = x.shape
     q = torch.empty(m, k, dtype=torch.float8_e4m3fn, device=x.device)
     s = torch.empty(k // 128, m, dtype=torch.float32, device=x.device)
-    L = _lib.load()
-    check(L.gllm_fp8_quant_group(_p(x), x.stride(0), _p(q), _p(s), m, k, stream_ptr()), "fp8_quant_group")
-    _count()
+    launch("gllm_fp8_quant_group", _p(x), x.stride(0), _p(q), _p(s), m, k)
     return q, s
 
 
@@ -617,10 +530,7 @@ def linear_fp8_block(x: torch.Tensor, w8: torch.Tensor, w_scale_inv: torch.Tenso
     if m == 0:
         return out
     xq, xs = fp8_quant_group(x)
-    L = _lib.load()
-    check(L.gllm_gemm_fp8_block(_p(xq), _p(xs), _p(w8), _p(w_scale_inv), _p(out), out.stride(0), m, n, k, _p(bias),
-                                stream_ptr()), "gemm_fp8_block")
-    _count()
+    launch("gllm_gemm_fp8_block", _p(xq), _p(xs), _p(w8), _p(w_scale_inv), _p(out), out.stride(0), m, n, k, _p(bias))
     return out
 
 
@@ -659,11 +569,8 @@ def mla_rope_cache(q_pe: torch.Tensor, q_full: torch.Tensor, k_pe: torch.Tensor,
     assert q_full.is_contiguous() and q_full.shape == (t, h, 576) and cos_sin.dtype == torch.float32
     if positions.dim() == 2:
         positions = positions[0]
-    L = _lib.load()
-    check(L.gllm_mla_rope_cache(_p(q_pe), q_pe.stride(0), q_pe.stride(1), h, _p(q_full), _p(k_pe), k_pe.stride(0),
-                                _p(kv_c), kv_c.stride(0), _p(cos_sin), _p(positions), _p(slots), _p(cache),
-                                cache.shape[3], t, stream_ptr()), "mla_rope_cache")
-    _count()
+    launch("gllm_mla_rope_cache", _p(q_pe), q_pe.stride(0), q_pe.stride(1), h, _p(q_full), _p(k_pe), k_pe.stride(0),
+           _p(kv_c), kv_c.stride(0), _p(cos_sin), _p(positions), _p(slots), _p(cache), cache.shape[3], t)
 
 
 def mla_attention(q_full: torch.Tensor, cache: torch.Tensor, block_table: torch.Tensor,
@@ -686,11 +593,9 @@ def mla_attention(q_full: torch.Tensor, cache: torch.Tensor, block_table: torch.
     if splits > 1:
         part_o, part_lse = _mla_workspace(q_full.device, h)
         assert t * h * splits <= part_lse.numel()
-    L = _lib.load()
-    check(L.gllm_mla_attention(_p(q_full), _p(out), _p(cache), pages, _p(block_table), _p(tok_seq), _p(positions),
-                               _p(part_o), _p(part_lse), t, block_table.shape[1], h, page_size, splits, float(scale),
-                               stream_ptr()), "mla_attention")
-    _count(2 if splits > 1 else 1)
+    launch("gllm_mla_attention", _p(q_full), _p(out), _p(cache), pages, _p(block_table), _p(tok_seq), _p(positions),
+           _p(part_o), _p(part_lse), t, block_table.shape[1], h, page_size, splits, float(scale),
+           n=2 if splits > 1 else 1)
     return out
 
 
@@ -714,10 +619,8 @@ def lora_shrink(x: torch.Tensor, A: torch.Tensor, slots: torch.Tensor, row_off: 
     u = torch.empty(t, m, dtype=torch.float32, device=x.device)
     splits = lora_k_splits(t, k, m)
     ws = torch.empty(splits * t * m, dtype=torch.float32, device=x.device) if splits > 1 else None
-    L = _lib.load()
-    check(L.gllm_lora_shrink(_p(x), x.stride(0), _p(A), _p(u), _p(ws), t, k, m, _p(slots), _p(row_off), _p(rows),
-                             num_groups, splits, stream_ptr()), "lora_shrink")
-    _count(2 if splits > 1 and num_groups > 0 else 1)
+    launch("gllm_lora_shrink", _p(x), x.stride(0), _p(A), _p(u), _p(ws), t, k, m, _p(slots), _p(row_off), _p(rows),
+           num_groups, splits, n=2 if splits > 1 and num_groups > 0 else 1)
     return u
 
 
@@ -728,11 +631,8 @@ def lora_expand_add(y: torch.Tensor, u: torch.Tensor, B: torch.Tensor, bounds, s
     assert u.dtype == torch.float32 and u.stride(1) == 1 and len(bounds) in (2, 3, 4) and bounds[-1] == y.shape[1]
     n, r = B.shape[1], B.shape[2]
     nb = list(bounds[1:-1]) + [n, n]
-    L = _lib.load()
-    check(L.gllm_lora_expand_add(_p(u), u.stride(0), _p(B), _p(y), y.stride(0), y.shape[0], n, r, nb[0], nb[1],
-                                 (len(bounds) - 1) * r, _p(slots), _p(row_off), _p(rows), num_groups, stream_ptr()),
-          "lora_expand_add")
-    _count()
+    launch("gllm_lora_expand_add", _p(u), u.stride(0), _p(B), _p(y), y.stride(0), y.shape[0], n, r, nb[0], nb[1],
+           (len(bounds) - 1) * r, _p(slots), _p(row_off), _p(rows), num_groups)
     return y
 
 
@@ -743,13 +643,6 @@ def lora_expand_silu_mul(pre: torch.Tensor, u: torch.Tensor, B: torch.Tensor, sl
     t, two_i = pre.shape
     r = B.shape[2]
     out = torch.empty(t, two_i // 2, dtype=_BF16, device=pre.device)
-    L = _lib.load()
-    check(L.gllm_lora_expand_silu_mul(_p(pre), pre.stride(0), _p(u), u.stride(0), _p(B), _p(out), out.stride(0), t,
-                                      two_i // 2, r, _p(slots), _p(row_off), _p(rows), num_groups, stream_ptr()),
-          "lora_expand_silu_mul")
-    _count()
+    launch("gllm_lora_expand_silu_mul", _p(pre), pre.stride(0), _p(u), u.stride(0), _p(B), _p(out), out.stride(0), t,
+           two_i // 2, r, _p(slots), _p(row_off), _p(rows), num_groups)
     return out
-
-
-# the MoE front-ends, so that a model module sees one table (sm100_moe imports _count and _p, defined above)
-from gllm_b200.ops.sm100_moe import fused_experts, fused_experts_fp8, grouped_topk, topk_softmax  # noqa: E402,F401

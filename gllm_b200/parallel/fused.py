@@ -16,54 +16,17 @@ Reference behaviour replaced: GEMM -> NCCL all_reduce -> fused_add_rms_norm on r
 """
 from __future__ import annotations
 
-import ctypes
 import os
-from ctypes import c_float, c_int, c_int64, c_uint32, c_void_p
 from typing import Optional
 
 import torch
 import torch.distributed as dist
 
 from gllm_b200.ops import lib as _lib
-from gllm_b200.ops.lib import MAX_PEERS, GemmComm, check, stream_ptr
+from gllm_b200.ops.lib import EpArgs, GemmComm, LLArgs, NvlsArgs, ReduceNormArgs, launch
 from gllm_b200.parallel import state as ps
 from gllm_b200.parallel.tp import TPComm
 from gllm_b200.utils.logging import logger
-
-
-class ReduceNormArgs(ctypes.Structure):
-    _fields_ = [
-        ("stage", c_void_p), ("cnt", c_void_p), ("n_tiles", c_uint32 * MAX_PEERS), ("local_x", c_void_p),
-        ("local_ld", c_int64), ("residual", c_void_p), ("residual_in", c_int), ("norm_w", c_void_p),
-        ("ag_peers", c_void_p * MAX_PEERS), ("flag_peers", c_void_p * MAX_PEERS), ("unnormed_out", c_void_p),
-        ("st", c_void_p), ("parity", c_int), ("ag_idx", c_int), ("tp", c_int), ("rank", c_int),
-        ("rows_per_rank", c_int), ("rows_valid", c_int), ("H", c_int), ("eps", c_float), ("T", c_int),
-        ("bcast", c_int), ("push_x", c_void_p), ("push_ld", c_int64), ("stage_peers", c_void_p * MAX_PEERS),
-        ("cnt_peers", c_void_p * MAX_PEERS),
-    ]
-
-
-class LLArgs(ctypes.Structure):
-    """Mirror of `LLArgs` in csrc/comm/tp_fused.cu (one-shot LL all-reduce + add + RMSNorm)."""
-    _fields_ = [("x", c_void_p), ("ldx", c_int64), ("residual", c_void_p), ("residual_in", c_int),
-                ("norm_w", c_void_p), ("out", c_void_p), ("ll_peers", c_void_p * MAX_PEERS), ("st", c_void_p),
-                ("tp", c_int), ("rank", c_int), ("T", c_int), ("H", c_int), ("row_cap", c_int), ("eps", c_float)]
-
-
-class NvlsArgs(ctypes.Structure):
-    """Mirror of `NvlsArgs` in csrc/comm/tp_fused.cu (in-switch multimem all-reduce + add + RMSNorm)."""
-    _fields_ = [("x", c_void_p), ("ldx", c_int64), ("residual", c_void_p), ("residual_in", c_int),
-                ("norm_w", c_void_p), ("out", c_void_p), ("buf_local", c_void_p), ("buf_mc", c_void_p),
-                ("flags_mc", c_void_p), ("flags_local", c_void_p), ("st", c_void_p),
-                ("tp", c_int), ("rank", c_int), ("T", c_int), ("H", c_int), ("row_cap", c_int), ("eps", c_float)]
-
-
-class EpArgs(ctypes.Structure):
-    """Mirror of `EpArgs` in csrc/comm/ep_a2a.cu."""
-    _fields_ = [("recv_x", c_void_p * MAX_PEERS), ("recv_e", c_void_p * MAX_PEERS),
-                ("recv_src", c_void_p * MAX_PEERS), ("ctrl", c_void_p * MAX_PEERS), ("comb", c_void_p * MAX_PEERS),
-                ("state", c_void_p), ("ep", c_int), ("rank", c_int), ("experts_per_rank", c_int), ("top_k", c_int),
-                ("H", c_int), ("r_max", c_int)]
 
 
 _ONESHOT = os.environ.get("GLLM_TP_ONESHOT", "1") != "0"
@@ -80,29 +43,6 @@ def small_threshold(tp: int) -> int:
     if _SMALL_T_ENV != "auto":
         return SMALL_T
     return max(8, min(SMALL_T, 112 // max(tp - 1, 1)))
-
-
-def _declare(L):
-    L.gllm_rs_reduce_norm.argtypes = [ctypes.POINTER(ReduceNormArgs), c_void_p]
-    L.gllm_rs_reduce_norm.restype = c_int
-    L.gllm_push_partial_rows.argtypes = [c_void_p, c_int64, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]
-    L.gllm_push_partial_rows.restype = c_int
-    L.gllm_wait_ag_flags.argtypes = [c_void_p, c_void_p, c_int, c_int, c_void_p]
-    L.gllm_wait_ag_flags.restype = c_int
-    L.gllm_tp_state_bytes.argtypes = []
-    L.gllm_tp_state_bytes.restype = c_int
-    L.gllm_ll_allreduce_norm.argtypes = [ctypes.POINTER(LLArgs), c_void_p]
-    L.gllm_ll_allreduce_norm.restype = c_int
-    L.gllm_nvls_allreduce_norm.argtypes = [ctypes.POINTER(NvlsArgs), c_void_p]
-    L.gllm_nvls_allreduce_norm.restype = c_int
-    L.gllm_ep_state_bytes.argtypes = []
-    L.gllm_ep_state_bytes.restype = c_int
-    L.gllm_ep_dispatch.argtypes = [ctypes.POINTER(EpArgs), c_void_p, c_int64, c_void_p, c_int, c_void_p]
-    L.gllm_ep_dispatch.restype = c_int
-    L.gllm_ep_row_dest.argtypes = [ctypes.POINTER(EpArgs), c_void_p, c_void_p, c_int, c_void_p]
-    L.gllm_ep_row_dest.restype = c_int
-    L.gllm_ep_combine.argtypes = [ctypes.POINTER(EpArgs), c_void_p, c_void_p, c_int, c_void_p]
-    L.gllm_ep_combine.restype = c_int
 
 
 class FusedTPComm(TPComm):
@@ -122,7 +62,6 @@ class FusedTPComm(TPComm):
         self.rpr_max = (max_tokens + tp - 1) // tp
         t_pad = self.rpr_max * tp
         L = _lib.load()
-        _declare(L)
         self.L = L
         # ---- one symmetric blob: [stage x2][ag x3][cnt x2][flags x3] ----
         stage_bytes = tp * self.rpr_max * hidden_size * 2
@@ -252,9 +191,7 @@ class FusedTPComm(TPComm):
             for p in range(self.tp_size):
                 a.stage_peers[p] = self.peer_base[p] + self.off_stage[parity]
                 a.cnt_peers[p] = self.peer_base[p] + self.off_cnt[parity]
-        check(self.L.gllm_rs_reduce_norm(ctypes.byref(a), stream_ptr()), "rs_reduce_norm")
-        from gllm_b200.ops import sm100
-        sm100._count()
+        launch("gllm_rs_reduce_norm", a)
         h = self._ag_view(ag_idx)
         if bcast:
             self.cur_ag = None  # all rows were written by this rank's own kernel: nothing to gate on
@@ -296,10 +233,7 @@ class FusedTPComm(TPComm):
         """Make the gather buffer safe to read by a kernel that does not understand the flags."""
         if not self.small and self.cur_ag is not None and h.data_ptr() == self.cur_ag[1].data_ptr():
             idx = self.cur_ag[0]
-            check(self.L.gllm_wait_ag_flags(self.local_base + self.off_flag[idx], self.state.data_ptr(), idx,
-                                            self.T, stream_ptr()), "wait_ag_flags")
-            from gllm_b200.ops import sm100
-            sm100._count()
+            launch("gllm_wait_ag_flags", self.local_base + self.off_flag[idx], self.state.data_ptr(), idx, self.T)
         return h
 
     def col_linear(self, x, w, bias=None):
@@ -346,7 +280,6 @@ class FusedTPComm(TPComm):
         return self._reduce_norm(parity, n_tiles, None, residual is not None, norm_w, eps, bcast=bcast)
 
     def reduce_add_norm(self, partial, residual, norm_w, eps):
-        from gllm_b200.ops import sm100
         if self.small:
             if not self.oneshot or partial.dtype != torch.bfloat16:
                 return super().reduce_add_norm(partial, residual, norm_w, eps)
@@ -372,8 +305,7 @@ class FusedTPComm(TPComm):
                 n.st = self.state.data_ptr()
                 n.tp, n.rank, n.T, n.H, n.row_cap, n.eps = (self.tp_size, self.tp_rank, self.T, self.H, SMALL_T,
                                                             float(eps))
-                check(self.L.gllm_nvls_allreduce_norm(ctypes.byref(n), stream_ptr()), "nvls_allreduce_norm")
-                sm100._count()
+                launch("gllm_nvls_allreduce_norm", n)
                 self.nvls_calls += 1
                 self.cur_ag = None
                 return h, self.residual_buf[: self.T]
@@ -385,17 +317,14 @@ class FusedTPComm(TPComm):
                 a.ll_peers[p] = self.peer_base[p] + self.off_ll[parity]
             a.st = self.state.data_ptr()
             a.tp, a.rank, a.T, a.H, a.row_cap, a.eps = self.tp_size, self.tp_rank, self.T, self.H, SMALL_T, float(eps)
-            check(self.L.gllm_ll_allreduce_norm(ctypes.byref(a), stream_ptr()), "ll_allreduce_norm")
-            sm100._count()
+            launch("gllm_ll_allreduce_norm", a)
             self.cur_ag = None
             return h, self.residual_buf[: self.T]
         parity = self.rs_call % 2
         self.rs_call += 1
         assert partial.shape[0] == self.T and partial.shape[1] == self.H and partial.stride(1) == 1
-        check(self.L.gllm_push_partial_rows(partial.data_ptr(), partial.stride(0), self.T, self.H, self.tp_rank,
-                                            self.rpr, self.stage_tbl[parity].data_ptr(),
-                                            self.cnt_tbl[parity].data_ptr(), stream_ptr()), "push_partial_rows")
-        sm100._count()
+        launch("gllm_push_partial_rows", partial.data_ptr(), partial.stride(0), self.T, self.H, self.tp_rank, self.rpr,
+               self.stage_tbl[parity].data_ptr(), self.cnt_tbl[parity].data_ptr())
         return self._reduce_norm(parity, self._rows_valid(), None, residual is not None, norm_w, eps)
 
     def close(self):
@@ -474,7 +403,7 @@ class FusedTPComm(TPComm):
         dispatch -> grouped GEMMs whose epilogue returns the rows -> combine, all over peer memory."""
         if not self.can_a2a(block):
             return super().moe_add_norm(block, h, residual, norm_w, eps)
-        from gllm_b200.ops import sm100, sm100_moe
+        from gllm_b200.ops import sm100_moe
         ex = block.experts
         if self.ep is None:
             self._ep_setup(ex)
@@ -484,29 +413,24 @@ class FusedTPComm(TPComm):
         self.ep_call += 1
         a = ep["args"][par]
         rv, r0 = self._rows_valid(), self.tp_rank * self.rpr
-        st = stream_ptr()
         if rv > 0:
             w, ids = ex.route(h[r0:r0 + rv])   # own rows of the gather buffer are local writes: no flag wait
             xs = h[r0:r0 + rv]
-            check(self.L.gllm_ep_dispatch(ctypes.byref(a), xs.data_ptr(), xs.stride(0), ids.data_ptr(), rv, st),
-                  "ep_dispatch")
+            launch("gllm_ep_dispatch", a, xs.data_ptr(), xs.stride(0), ids.data_ptr(), rv, n=0)
         else:
             w = None
-            check(self.L.gllm_ep_dispatch(ctypes.byref(a), None, 0, None, 0, st), "ep_dispatch")
+            launch("gllm_ep_dispatch", a, None, 0, None, 0, n=0)
 
         def row_dest_fn(slot_pos, rows):
             rd = ep["row_dest"]
             assert rows <= rd.numel()
-            check(self.L.gllm_ep_row_dest(ctypes.byref(a), slot_pos.data_ptr(), rd.data_ptr(), rows, st),
-                  "ep_row_dest")
+            launch("gllm_ep_row_dest", a, slot_pos.data_ptr(), rd.data_ptr(), rows, n=0)
             return rd
 
         sm100_moe.fused_experts(ep["recv_x"][par], ex.w13, ex.w2, None, ep["recv_e"][par], None,
                                 n_valid=ep["n_valid"][par], row_dest_fn=row_dest_fn)
         out = ep["out"]
-        check(self.L.gllm_ep_combine(ctypes.byref(a), w.data_ptr() if w is not None else None, out.data_ptr(), rv,
-                                     st), "ep_combine")
-        sm100._count(6)
+        launch("gllm_ep_combine", a, w.data_ptr() if w is not None else None, out.data_ptr(), rv, n=6)
         # `out` holds this rank's rows only; rs_reduce_norm indexes a full [T, H] tensor by global row
         shifted = _ShiftedRows(out, r0)
         return self._reduce_norm(0, 0, shifted, residual is not None, norm_w, eps)
