@@ -47,6 +47,7 @@ class EngineConfig:
     tokenizer_path: Optional[str] = None
     lora_modules: Optional[Dict[str, str]] = None   # multi-LoRA: adapter name -> PEFT directory (gllm_b200/lora.py)
     max_lora_rank: int = 16                           # every adapter is zero-padded to this rank (<= 64)
+    quantization: Optional[str] = None        # "fp8": quantise a 16-bit checkpoint's linears to FP8 W8A8 at load
 
     @property
     def world_size(self) -> int:

@@ -12,7 +12,14 @@
 // warpgroups own 64 rows each of the 128 x 128 tile. Same TMA (SWIZZLE_128B, 128 fp8 = one 128-byte row) /
 // mbarrier ring as gemm_bf16.cu.
 //
-// Also here: the dynamic per-token-group activation quantiser (reference fp8.py:354-552).
+// The same kernel, instantiated with kW8A8 = true, is the large-M W8A8 GEMM of per-channel / per-tensor FP8
+// checkpoints: a_s fp32 [M] (one scale per token), w_s fp32 [N] (one per output channel). Each 128-deep K block is
+// promoted unscaled (acc += partial, since wgmma's e4m3 accumulator keeps fewer bits than fp32) and the epilogue
+// applies y = bf16(acc * a_s[m] * w_s[n] + bias[n]). K only needs to be a multiple of 16 (the TMA row pitch): the
+// last K block is zero-filled by TMA.
+//
+// Also here: the dynamic per-token-group activation quantiser (reference fp8.py:354-552) and the per-token one of
+// the W8A8 path.
 #include <cuda_fp8.h>
 #include <string.h>
 
@@ -29,9 +36,9 @@ struct Fp8Params {
   int M, N, K;
   __nv_bfloat16* C;
   int ldc;
-  const float* a_s;  // [K/128, M]
+  const float* a_s;  // [K/128, M]  (W8A8: [M])
   int lda_s;         // = M (row pitch of a_s)
-  const float* w_s;  // [N/128, K/128]  (grouped: [E][N/64][K/128], one scale row per 64 weight rows)
+  const float* w_s;  // [N/128, K/128]  (grouped: [E][N/64][K/128], one scale row per 64 weight rows; W8A8: [N])
   const __nv_bfloat16* bias;
   // grouped (MoE) mode: M tile t multiplies the e4m3 slab of expert tile_expert[t]; the weight scales are
   // stored per 64-row half tile so a [64 gate | 64 up] interleaved tile can carry two different block scales
@@ -42,6 +49,7 @@ struct Fp8Params {
   int silu;              // 1: out[:, j] = silu(acc[j]) * acc[64 + j]  (64 output columns per tile)
 };
 
+template <bool kW8A8>
 __global__ void __launch_bounds__(kFThreads, 1)
 gemm_fp8_block_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                       const Fp8Params p) {
@@ -57,7 +65,7 @@ gemm_fp8_block_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_c
                                                  : (p.M + kFBM - 1) / kFBM;
   const int num_n = (p.N + kFBN - 1) / kFBN;
   const int num_tiles = num_m * num_n;
-  const int num_kb = p.K / kFBK;
+  const int num_kb = kW8A8 ? (p.K + kFBK - 1) / kFBK : p.K / kFBK;
 
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&tmap_a);
@@ -108,6 +116,14 @@ gemm_fp8_block_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_c
         for (int k = 0; k < kFBK / 32; ++k)  // K = 32 for 8-bit operands: +32 B per step
           wgmma_e4m3_ss<kFBN>(part, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), k > 0 ? 1u : 0u);
         wgmma_commit();
+        if constexpr (kW8A8) {
+          wgmma_wait<0>();
+          reg_fence(part);
+          if (lane == 0) mbar_arrive(&empty_bar[s]);
+#pragma unroll
+          for (int i = 0; i < kFBN / 2; ++i) acc[i] += part[i];
+          continue;
+        }
         // scales of this K block load while the tensor core runs
         const float sa0 = row0 < p.M ? p.a_s[static_cast<size_t>(kb) * p.lda_s + row0] : 0.f;
         const float sa1 = row1 < p.M ? p.a_s[static_cast<size_t>(kb) * p.lda_s + row1] : 0.f;
@@ -137,7 +153,23 @@ gemm_fp8_block_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_c
         const int row = h ? row1 : row0;
         if (row >= p.M) continue;
         __nv_bfloat16* crow = p.C + static_cast<size_t>(row) * p.ldc;
-        if (p.silu) {
+        if constexpr (kW8A8) {
+          const float sx = p.a_s[row];
+#pragma unroll
+          for (int j = 0; j < kFBN / 8; ++j) {
+            const int col = n0 + 8 * j + cq;
+            if (col < p.N) {
+              const float2 sw = *reinterpret_cast<const float2*>(p.w_s + col);
+              float f0 = __fmul_rn(__fmul_rn(acc[4 * j + 2 * h], sx), sw.x);
+              float f1 = __fmul_rn(__fmul_rn(acc[4 * j + 2 * h + 1], sx), sw.y);
+              if (p.bias != nullptr) {
+                const float2 bv = unpack_bf16(*reinterpret_cast<const uint32_t*>(p.bias + col));
+                f0 = __fadd_rn(f0, bv.x); f1 = __fadd_rn(f1, bv.y);
+              }
+              *reinterpret_cast<uint32_t*>(crow + col) = pack_bf16(f0, f1);
+            }
+          }
+        } else if (p.silu) {
 #pragma unroll
           for (int j = 0; j < 8; ++j) {
             const int col = n0 / 2 + 8 * j + cq;
@@ -194,6 +226,77 @@ __global__ void fp8_quant_group_kernel(const __nv_bfloat16* __restrict__ x, int6
   if (lane == 0) scales[static_cast<size_t>(g) * M + row] = scale;
 }
 
+// Per-token quantisation of the W8A8 path: x bf16 [M, K] (row stride ldx) -> q e4m3 [M, K] contiguous, s fp32 [M].
+// One CTA per row. Dynamic (static_scale == nullptr): s = max(amax |x|, 1e-10) / 448 and q = e4m3_rn(x * (1 / s)),
+// the reciprocal taken first. Static: s = *static_scale and q = e4m3_rn(clamp(x / s, +-448)). Every division is
+// correctly rounded (the library builds with fast math), so ops.ref.fp8_quant_token gives the same bits.
+static constexpr int kQThreads = 256;
+
+__device__ __forceinline__ __nv_fp8_e4m3 to_e4m3(float v) {
+  __nv_fp8_e4m3 r;
+  r.__x = __nv_cvt_float_to_fp8(v, __NV_SATFINITE, __NV_E4M3);
+  return r;
+}
+
+template <bool kVec>   // kVec: K, ldx and x 16-byte aligned: 8 elements per load
+__global__ void __launch_bounds__(kQThreads)
+fp8_quant_token_kernel(const __nv_bfloat16* __restrict__ x, int64_t ldx, __nv_fp8_e4m3* __restrict__ q,
+                       float* __restrict__ scales, const float* __restrict__ static_scale, int K) {
+  __shared__ float red[kQThreads / 32];
+  const int row = blockIdx.x;
+  const __nv_bfloat16* src = x + static_cast<size_t>(row) * ldx;
+  __nv_fp8_e4m3* dst = q + static_cast<size_t>(row) * K;
+  float s;
+  if (static_scale != nullptr) {
+    s = *static_scale;
+  } else {
+    float amax = 0.f;
+    if constexpr (kVec) {
+      for (int k = threadIdx.x * 8; k < K; k += kQThreads * 8) {
+        const uint4 raw = *reinterpret_cast<const uint4*>(src + k);
+        const uint32_t w[4] = {raw.x, raw.y, raw.z, raw.w};
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const float2 f = unpack_bf16(w[i]);
+          amax = fmaxf(amax, fmaxf(fabsf(f.x), fabsf(f.y)));
+        }
+      }
+    } else {
+      for (int k = threadIdx.x; k < K; k += kQThreads) amax = fmaxf(amax, fabsf(__bfloat162float(src[k])));
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = amax;
+    __syncthreads();
+    amax = red[0];
+#pragma unroll
+    for (int i = 1; i < kQThreads / 32; ++i) amax = fmaxf(amax, red[i]);
+    s = __fdiv_rn(fmaxf(amax, 1e-10f), 448.f);
+  }
+  const bool dyn = static_scale == nullptr;
+  const float inv = __frcp_rn(s);
+  auto quant = [&](float v) {
+    return to_e4m3(dyn ? __fmul_rn(v, inv) : fminf(fmaxf(__fdiv_rn(v, s), -448.f), 448.f));
+  };
+  if constexpr (kVec) {
+    for (int k = threadIdx.x * 8; k < K; k += kQThreads * 8) {
+      const uint4 raw = *reinterpret_cast<const uint4*>(src + k);
+      const uint32_t w[4] = {raw.x, raw.y, raw.z, raw.w};
+      __nv_fp8_e4m3 o[8];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const float2 f = unpack_bf16(w[i]);
+        o[2 * i] = quant(f.x);
+        o[2 * i + 1] = quant(f.y);
+      }
+      *reinterpret_cast<uint2*>(dst + k) = *reinterpret_cast<const uint2*>(o);
+    }
+  } else {
+    for (int k = threadIdx.x; k < K; k += kQThreads) dst[k] = quant(__bfloat162float(src[k]));
+  }
+  if (threadIdx.x == 0) scales[row] = s;
+}
+
 }  // namespace b200
 
 using namespace b200;
@@ -232,12 +335,12 @@ GLLM_EXPORT int gllm_gemm_fp8_block(const void* A8, const void* a_s, const void*
   constexpr int smem_bytes = kFStages * (kFBM * kFBK + kFBN * kFBK) + 1024 + 256;
   static PerDeviceOnce configured;
   if (configured.need()) {
-    CUDA_CHECK_RET(cudaFuncSetAttribute(gemm_fp8_block_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
+    CUDA_CHECK_RET(cudaFuncSetAttribute(gemm_fp8_block_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
     configured.done();
   }
   const int tiles = ((M + kFBM - 1) / kFBM) * ((N + kFBN - 1) / kFBN);
   const int grid = tiles < num_sms() ? tiles : num_sms();
-  gemm_fp8_block_kernel<<<grid, kFThreads, smem_bytes, reinterpret_cast<cudaStream_t>(stream)>>>(ta, tb, p);
+  gemm_fp8_block_kernel<false><<<grid, kFThreads, smem_bytes, reinterpret_cast<cudaStream_t>(stream)>>>(ta, tb, p);
   CUDA_CHECK_RET(cudaGetLastError());
   return 0;
 }
@@ -271,10 +374,58 @@ GLLM_EXPORT int gllm_moe_grouped_gemm_fp8(const void* A8, const void* a_s, const
   p.ws_stride_e = static_cast<int64_t>(N / 64) * (K / 128);
   p.silu = epi == 1 ? 1 : 0;
   constexpr int smem_bytes = kFStages * (kFBM * kFBK + kFBN * kFBK) + 1024 + 256;
-  CUDA_CHECK_RET(cudaFuncSetAttribute(gemm_fp8_block_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
+  CUDA_CHECK_RET(cudaFuncSetAttribute(gemm_fp8_block_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
   const int tiles = max_tiles * (N / kFBN);
   const int grid = tiles < num_sms() ? tiles : num_sms();
-  gemm_fp8_block_kernel<<<grid, kFThreads, smem_bytes, reinterpret_cast<cudaStream_t>(stream)>>>(ta, tb, p);
+  gemm_fp8_block_kernel<false><<<grid, kFThreads, smem_bytes, reinterpret_cast<cudaStream_t>(stream)>>>(ta, tb, p);
+  CUDA_CHECK_RET(cudaGetLastError());
+  return 0;
+}
+
+// x bf16 [M, K] (row stride ldx) -> q e4m3 [M, K] contiguous, s fp32 [M]; static_scale: fp32 scalar or null (dynamic)
+GLLM_EXPORT int gllm_fp8_quant_token(const void* x, int64_t ldx, void* q, void* scales, const void* static_scale, int M,
+                                     int K, void* stream) {
+  if (M <= 0) return 0;
+  const bool vec = K % 8 == 0 && ldx % 8 == 0 && reinterpret_cast<uintptr_t>(x) % 16 == 0;
+  auto kern = vec ? fp8_quant_token_kernel<true> : fp8_quant_token_kernel<false>;
+  kern<<<M, kQThreads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      reinterpret_cast<const __nv_bfloat16*>(x), ldx, reinterpret_cast<__nv_fp8_e4m3*>(q),
+      reinterpret_cast<float*>(scales), reinterpret_cast<const float*>(static_scale), K);
+  CUDA_CHECK_RET(cudaGetLastError());
+  return 0;
+}
+
+// Large-M W8A8 GEMM: A8 [M, K] e4m3 contiguous with per-token scales a_s fp32 [M]; W8 [N, K] e4m3 contiguous with
+// per-channel scales w_s fp32 [N]. C[m, n] = bf16(acc * a_s[m] * w_s[n] + bias[n]).
+GLLM_EXPORT int gllm_gemm_fp8_w8a8(const void* A8, const void* a_s, const void* W8, const void* w_s, void* C,
+                                   int64_t ldc, int M, int N, int K, const void* bias, void* stream) {
+  if (M <= 0 || N <= 0) return 0;
+  if (K % 16 != 0 || N % 8 != 0 || ldc % 2 != 0) {
+    fprintf(stderr, "[gllm_b200] gemm_fp8_w8a8: K %% 16, N %% 8 and even ldc required (M=%d N=%d K=%d)\n", M, N, K);
+    return 1;
+  }
+  CUtensorMap ta, tb;
+  if (make_tmap_2d(&ta, A8, M, K, K, kFBM, kFBK, CU_TENSOR_MAP_DATA_TYPE_UINT8)) return 1;
+  if (make_tmap_2d(&tb, W8, N, K, K, kFBN, kFBK, CU_TENSOR_MAP_DATA_TYPE_UINT8)) return 1;
+  Fp8Params p;
+  memset(&p, 0, sizeof(p));
+  p.M = M; p.N = N; p.K = K;
+  p.C = reinterpret_cast<__nv_bfloat16*>(C);
+  p.ldc = static_cast<int>(ldc);
+  p.a_s = reinterpret_cast<const float*>(a_s);
+  p.lda_s = M;
+  p.w_s = reinterpret_cast<const float*>(w_s);
+  p.bias = reinterpret_cast<const __nv_bfloat16*>(bias);
+  constexpr int smem_bytes = kFStages * (kFBM * kFBK + kFBN * kFBK) + 1024 + 256;
+  static PerDeviceOnce configured;
+  if (configured.need()) {
+    CUDA_CHECK_RET(cudaFuncSetAttribute(gemm_fp8_block_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        smem_bytes));
+    configured.done();
+  }
+  const int tiles = ((M + kFBM - 1) / kFBM) * ((N + kFBN - 1) / kFBN);
+  const int grid = tiles < num_sms() ? tiles : num_sms();
+  gemm_fp8_block_kernel<true><<<grid, kFThreads, smem_bytes, reinterpret_cast<cudaStream_t>(stream)>>>(ta, tb, p);
   CUDA_CHECK_RET(cudaGetLastError());
   return 0;
 }

@@ -158,7 +158,7 @@ class LLM:
             model_max_length=model_max_length, mm_processor_min_pixels=mm_processor_min_pixels,
             mm_processor_max_pixels=mm_processor_max_pixels, **extra)
         cfg = self.cfg
-        self.loader = ModelLoader(cfg.model_path, cfg.load_format)
+        self.loader = ModelLoader(cfg.model_path, cfg.load_format, cfg.quantization)
         from gllm_b200.lora import adapter_ids
         # multi-LoRA: adapter name -> id (0 is the base model), validated before any worker starts
         self.lora_ids: Dict[str, int] = adapter_ids(self.loader.architecture, cfg.lora_modules, cfg.max_lora_rank)

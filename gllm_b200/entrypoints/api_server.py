@@ -501,6 +501,9 @@ def make_parser() -> argparse.ArgumentParser:
     p.add_argument("--lora-modules", type=str, nargs="+", default=None, metavar="NAME=PATH",
                    help="PEFT LoRA adapters served next to the base model; a request selects one by `model`")
     p.add_argument("--max-lora-rank", type=int, default=16, help="every adapter is zero-padded to this rank (<= 64)")
+    p.add_argument("--quantization", type=str, choices=["fp8"], default=None,
+                   help="fp8: quantise a 16-bit checkpoint's linears to FP8 W8A8 at load (per-channel weights, "
+                        "per-token activations)")
     return p
 
 
@@ -530,7 +533,8 @@ def engine_kwargs(args) -> dict:
                 max_cuda_graph_bs=args.max_cuda_graph_bs, model_max_length=args.model_max_length,
                 mm_processor_min_pixels=args.mm_processor_min_pixels,
                 mm_processor_max_pixels=args.mm_processor_max_pixels, tp_mode=args.tp_mode,
-                lora_modules=parse_lora_modules(args.lora_modules), max_lora_rank=args.max_lora_rank)
+                lora_modules=parse_lora_modules(args.lora_modules), max_lora_rank=args.max_lora_rank,
+                quantization=args.quantization)
 
 
 async def run_server(app, host: str, port: int):

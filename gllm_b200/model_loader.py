@@ -19,10 +19,12 @@ from gllm_b200.utils.logging import logger
 
 
 class ModelLoader:
-    def __init__(self, model_path, load_format: str = "auto"):
+    def __init__(self, model_path, load_format: str = "auto", quantization: Optional[str] = None):
         self.model_path = model_path
         self.load_format = load_format
         self.config = self.load_config(model_path)
+        if quantization is not None:     # validated with the checkpoint's own config by registry.build_model
+            self.config[registry.QUANTIZATION_KEY] = quantization
         self.generation_config = self.load_generation_config(model_path)
         self.architecture = self.config["architectures"][0]
         self.use_mla = self.architecture in ("DeepseekV2ForCausalLM", "DeepseekV3ForCausalLM") and \

@@ -99,7 +99,7 @@ def _entry(vals: np.ndarray, ids: np.ndarray, j: int, n: int):
 class ModelRunner:
     def __init__(self, cfg: EngineConfig, loader: Optional[ModelLoader] = None):
         self.cfg = cfg
-        self.loader = loader or ModelLoader(cfg.model_path, cfg.load_format)
+        self.loader = loader or ModelLoader(cfg.model_path, cfg.load_format, cfg.quantization)
         self.page_size = cfg.page_size
         self.max_num_batched_tokens = cfg.max_num_batched_tokens
         self.max_running_seqs = cfg.max_running_seqs
@@ -142,8 +142,8 @@ class ModelRunner:
         self.spec = self.model.spec
         want_fused = cfg.tp_mode == "fused" and cfg.tp_size > 1 and is_cuda
         quant = getattr(self.spec, "quant", None)
-        why_not = {"fp8": "fp8 block-scaled linears", "awq": "AWQ int4 linears",
-                   "gptq": "GPTQ int4 linears"}.get(quant, quant) if quant is not None else \
+        why_not = {"fp8": "fp8 block-scaled linears", "awq": "AWQ int4 linears", "gptq": "GPTQ int4 linears",
+                   "w8a8": "FP8 W8A8 linears"}.get(quant, quant) if quant is not None else \
             "DeepStack (Qwen3-VL) feature injection" if getattr(self.model, "num_deepstack", 0) else \
             "LoRA adapters" if cfg.lora_modules else None
         if want_fused and why_not:

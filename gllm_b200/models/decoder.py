@@ -76,8 +76,10 @@ class ModelSpec:
     eos_token_id: Optional[object] = None
     extra: dict = field(default_factory=dict)
     quant: Optional[str] = None  # "fp8": block-scaled e4m3 linears (HF quantization_config, 128x128 blocks);
-    #                              "awq" / "gptq": int4 q/k/v/o/gate/up/down with group scales (`w4`)
+    #                              "awq" / "gptq": int4 q/k/v/o/gate/up/down with group scales (`w4`);
+    #                              "w8a8": e4m3 q/k/v/o/gate/up/down with per-channel scales (`w8`)
     w4: Optional[wu.W4Config] = None
+    w8: Optional[wu.W8Config] = None
 
     def is_moe_layer(self, layer_id: int) -> bool:
         if self.moe is None:
@@ -125,9 +127,25 @@ class W4Params(nn.Module):
         self.zeros = nn.Parameter(torch.zeros(g, np_, dtype=torch.uint8, device=device), requires_grad=False)
 
 
+class W8Params(nn.Module):
+    """Per-output-channel scales fp32 [n] of a W8A8 linear (its e4m3 codes are the `*_w` parameter beside it), and the
+    static activation scale (fp32 scalar) when the checkpoint has one."""
+
+    def __init__(self, n: int, cfg: wu.W8Config, device):
+        super().__init__()
+        self.scale = nn.Parameter(torch.ones(n, dtype=torch.float32, device=device), requires_grad=False)
+        self.input_scale = nn.Parameter(torch.ones((), dtype=torch.float32, device=device),
+                                        requires_grad=False) if cfg.static else None
+
+
 def _linear_params(n: int, k: int, spec: ModelSpec, device):
     """(weight, scale_inv | None): bf16 [n, k], or e4m3 [n, k] + fp32 block scales for fp8 checkpoints, or packed
-    int4 codes + `W4Params` for AWQ / GPTQ checkpoints."""
+    int4 codes + `W4Params` for AWQ / GPTQ checkpoints, or e4m3 [n, k] + `W8Params` for W8A8."""
+    if spec.w8 is not None:
+        if k % 16:
+            raise ValueError(f"FP8 W8A8: a linear's per-rank input width {k} is not a multiple of 16")
+        w = nn.Parameter(torch.zeros(n, k, dtype=torch.float8_e4m3fn, device=device), requires_grad=False)
+        return w, W8Params(n, spec.w8, device)
     if spec.w4 is not None:
         assert k % 32 == 0 and n % 8 == 0, (n, k)
         w = nn.Parameter(torch.zeros(-(-n // 16) * 16, -(-k // ref.W4_BLOCK_K) * ref.W4_BLOCK_K // 8,
@@ -145,6 +163,8 @@ def _qw(w, s):
     """Weight handle passed to the linear ops: plain tensor, (e4m3, scale_inv) for fp8, `Int4Weight` for int4."""
     if isinstance(s, W4Params):
         return ref.Int4Weight(w, s.scales, s.zeros, s.group_size, s.in_features)
+    if isinstance(s, W8Params):
+        return ref.Fp8Weight(w, s.scale, s.input_scale)
     return w if s is None else (w, s)
 
 
@@ -159,6 +179,13 @@ def _store_linear(w_param, s_param, w):
         if s_param.scales.dtype != scales.dtype:     # the checkpoint's 16-bit dtype is kept exactly
             s_param.scales.data = torch.empty_like(s_param.scales, dtype=scales.dtype)
         s_param.scales.data.copy_(scales)
+        return
+    if isinstance(w, wu.W8Tensor):      # codes and scales as they are: nothing is re-quantised
+        assert w.codes.shape == w_param.shape and w.scale.shape == s_param.scale.shape, (w.codes.shape, w_param.shape)
+        w_param.data.copy_(w.codes)
+        s_param.scale.data.copy_(w.scale)
+        if s_param.input_scale is not None:
+            s_param.input_scale.data.copy_(w.input_scale)
         return
     if s_param is None:
         w_param.data.copy_(w)
@@ -473,6 +500,10 @@ class CausalLM(nn.Module):
                 p.data.fill_(8)
             elif name.endswith("_ws.scales"):
                 p.data.fill_(0.02 / 21.5 ** 0.5)   # std of q - 8 over uniform codes is sqrt(21.5): weight std 0.02
+            elif name.endswith("_ws.scale"):
+                p.data.fill_(0.02 / 100.0)         # W8A8: e4m3 codes below have std about 100: weight std 0.02
+            elif name.endswith("_ws.input_scale"):
+                p.data.fill_(4.0 / 448.0)          # static activations: |x| up to 4 after RMSNorm
             elif name.endswith("norm_w"):
                 p.data.fill_(1.0)
             elif p.dim() == 1:
@@ -541,6 +572,8 @@ class CausalLM(nn.Module):
         """`<module>.weight`, or the module's int4 codes, zeros and scales (`W4Tensor`) for AWQ / GPTQ."""
         if self.spec.w4 is not None:
             return reader.get_w4(module, self.spec.w4)
+        if self.spec.w8 is not None:
+            return reader.get_w8(module, self.spec.w8)
         return reader.get(module + ".weight")
 
     def _load_attention(self, reader, pre, nm, at: Attention):
@@ -554,6 +587,9 @@ class CausalLM(nn.Module):
             qkv = wu.W4Tensor(*(
                 wu.shard_qkv(getattr(q, f), getattr(k, f), getattr(v, f), spec.num_heads, spec.num_kv_heads, d, tr,
                              tp) for f in ("codes", "zeros", "scales")))
+        elif isinstance(q, wu.W8Tensor):
+            qkv = wu.fuse_w8((q, k, v), lambda a, b, c: wu.shard_qkv(a, b, c, spec.num_heads, spec.num_kv_heads, d,
+                                                                      tr, tp))
         else:
             qkv = wu.shard_qkv(q, k, v, spec.num_heads, spec.num_kv_heads, d, tr, tp)
         _store_linear(at.qkv_w, at.qkv_ws, qkv)
@@ -581,6 +617,8 @@ class CausalLM(nn.Module):
         if isinstance(gate, wu.W4Tensor):
             mlp.set_gate_up(wu.W4Tensor(*(wu.shard_gate_up(getattr(gate, f), getattr(up, f), tr, tp)
                                           for f in ("codes", "zeros", "scales"))))
+        elif isinstance(gate, wu.W8Tensor):
+            mlp.set_gate_up(wu.fuse_w8((gate, up), lambda a, b: wu.shard_gate_up(a, b, tr, tp)))
         else:
             mlp.set_gate_up(wu.shard_gate_up(gate, up, tr, tp))
         _store_linear(mlp.down_w, mlp.down_ws, self._shard_cols(self._linear_weight(reader, pre + nm["down"])))
@@ -588,4 +626,6 @@ class CausalLM(nn.Module):
     def _shard_cols(self, w):
         if isinstance(w, wu.W4Tensor):
             return wu.shard_cols_w4(w, self.tp_rank, self.tp_size)
+        if isinstance(w, wu.W8Tensor):
+            return wu.shard_cols_w8(w, self.tp_rank, self.tp_size)
         return wu.shard_cols(w, self.tp_rank, self.tp_size)

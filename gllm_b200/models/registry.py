@@ -15,6 +15,9 @@ import torch
 from gllm_b200.models import weight_utils as wu
 from gllm_b200.models.decoder import CausalLM, ModelSpec, MoESpec
 
+# config key under which the engine's `quantization` option reaches the model builders (not an HF config key)
+QUANTIZATION_KEY = "gllm_quantization"
+
 _DTYPES = {"bfloat16": torch.bfloat16, "float16": torch.float16, "float32": torch.float32,
            torch.bfloat16: torch.bfloat16, torch.float16: torch.float16, torch.float32: torch.float32}
 
@@ -61,6 +64,11 @@ def _base_spec(cfg: HFConfig, arch: str, **kw) -> ModelSpec:
     if qc.get("quant_method") == "fp8" and list(qc.get("weight_block_size") or []) == [128, 128]:
         spec.quant = "fp8"
     spec.w4 = wu.w4_config(qc)
+    spec.w8 = wu.w8_config(qc, cfg.get(QUANTIZATION_KEY))
+    if spec.w8 is not None:
+        spec.quant = "w8a8"
+        if spec.dtype == torch.float16:
+            spec.dtype = torch.bfloat16
     if spec.w4 is not None:
         spec.quant = spec.w4.method
         if spec.dtype == torch.float16:    # every kernel here is bf16: fp16 tensors are rounded to bf16 once, at load
@@ -189,7 +197,11 @@ def build_model(cfg: HFConfig, device):
     arch = cfg["architectures"][0]
     if arch not in ARCHITECTURES:
         raise ValueError(f"unsupported architecture {arch}; supported: {sorted(ARCHITECTURES)}")
-    if wu.w4_config(cfg.get("quantization_config") or {}) is not None and arch not in wu.W4_ARCHITECTURES:
+    qc = cfg.get("quantization_config") or {}
+    if wu.w4_config(qc) is not None and arch not in wu.W4_ARCHITECTURES:
         raise ValueError(f"4-bit AWQ / GPTQ weights are not supported for {arch} (supported: "
+                         f"{', '.join(wu.W4_ARCHITECTURES)})")
+    if wu.w8_config(qc, cfg.get(QUANTIZATION_KEY)) is not None and arch not in wu.W4_ARCHITECTURES:
+        raise ValueError(f"FP8 W8A8 weights are not supported for {arch} (supported: "
                          f"{', '.join(wu.W4_ARCHITECTURES)})")
     return ARCHITECTURES[arch](cfg, device)

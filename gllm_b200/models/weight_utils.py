@@ -118,7 +118,7 @@ def w4_config(qc: dict) -> Optional[W4Config]:
     """Parse `quantization_config`: None for an unquantised or fp8 checkpoint, a `W4Config` for a supported AWQ /
     GPTQ one; anything else raises ValueError naming the cause."""
     method = str(qc.get("quant_method", "")).lower() if qc else ""
-    if method in ("", "fp8"):
+    if method in ("", "fp8", "compressed-tensors"):
         return None
     if method not in ("awq", "gptq"):
         raise ValueError(f"quantization method {method!r} is not supported (supported: fp8, awq, gptq)")
@@ -184,6 +184,100 @@ def shard_cols_w4(w: W4Tensor, rank: int, size: int) -> W4Tensor:
     one = w.zeros.shape[1] == 1 and w.codes.shape[1] > 1
     return W4Tensor(shard_cols(w.codes, rank, size), w.zeros if one else shard_cols(w.zeros, rank, size),
                     w.scales if one else shard_cols(w.scales, rank, size))
+
+
+# ------------------------------------------------------------------------------------------------
+# FP8 W8A8 checkpoints: per-channel / per-tensor e4m3 weights, per-token or static e4m3 activations
+# ------------------------------------------------------------------------------------------------
+@dataclass
+class W8Config:
+    """A validated W8A8 configuration. `method`: "fp8" (HF per-tensor), "compressed-tensors" or "fp8-online" (a 16-bit
+    checkpoint quantised per output channel at load); `static`: the checkpoint holds per-tensor `input_scale`s."""
+    method: str
+    static: bool = False
+
+
+def w8_config(qc: dict, quantization: Optional[str] = None) -> Optional[W8Config]:
+    """Parse `quantization_config` (and the engine's `quantization` option) into a `W8Config`: None when the checkpoint
+    is not a per-channel / per-tensor FP8 one; a ValueError naming the cause for an FP8 configuration this engine
+    cannot serve exactly."""
+    method = str(qc.get("quant_method", "")).lower() if qc else ""
+    if quantization is not None:
+        if quantization != "fp8":
+            raise ValueError(f"quantization={quantization!r} is not supported (None or 'fp8')")
+        if qc:
+            raise ValueError(f"quantization='fp8' needs an unquantised checkpoint; this one has a quantization_config "
+                             f"({method or qc})")
+        return W8Config("fp8-online")
+    if method == "fp8":
+        if qc.get("weight_block_size") is not None:     # block-scaled: de-quantised by `CheckpointReader.get`
+            return None
+        scheme = str(qc.get("activation_scheme", "dynamic")).lower()
+        if scheme not in ("dynamic", "static"):
+            raise ValueError(f"fp8: activation_scheme={scheme!r} is not supported ('dynamic' or 'static')")
+        _check_ignore("fp8", qc.get("ignored_layers") or qc.get("modules_to_not_convert") or [])
+        return W8Config("fp8", scheme == "static")
+    if method != "compressed-tensors":
+        return None
+    fmt = qc.get("format")
+    if fmt not in ("float-quantized", "naive-quantized"):
+        raise ValueError(f"compressed-tensors: format={fmt!r} is not supported ('float-quantized' or "
+                         f"'naive-quantized')")
+    groups = qc.get("config_groups") or {}
+    if len(groups) != 1:
+        raise ValueError(f"compressed-tensors: {len(groups)} config groups (exactly one, targeting Linear)")
+    grp = next(iter(groups.values()))
+    if list(grp.get("targets") or []) != ["Linear"]:
+        raise ValueError(f"compressed-tensors: targets={grp.get('targets')} is not supported (['Linear'])")
+    w, a = grp.get("weights") or {}, grp.get("input_activations")
+    if (w.get("num_bits"), str(w.get("type")), bool(w.get("symmetric", True))) != (8, "float", True):
+        raise ValueError(f"compressed-tensors: weights {w} are not 8-bit symmetric float")
+    if w.get("strategy") not in ("channel", "tensor"):
+        raise ValueError(f"compressed-tensors: weight strategy={w.get('strategy')!r} is not supported ('channel' or "
+                         f"'tensor')")
+    if w.get("dynamic", False):
+        raise ValueError("compressed-tensors: dynamic weight scales are not supported")
+    if a is None:
+        raise ValueError("compressed-tensors: weight-only FP8 (input_activations: null) is not supported")
+    if (a.get("num_bits"), str(a.get("type"))) != (8, "float"):
+        raise ValueError(f"compressed-tensors: input activations {a} are not 8-bit float")
+    act = (a.get("strategy"), bool(a.get("dynamic")))
+    if act not in (("token", True), ("tensor", False)):
+        raise ValueError(f"compressed-tensors: input activation strategy={act[0]!r}, dynamic={act[1]} is not "
+                         f"supported (token and dynamic, or tensor and static)")
+    _check_ignore("compressed-tensors", qc.get("ignore") or [])
+    if qc.get("kv_cache_scheme"):
+        from gllm_b200.utils.logging import logger
+        logger.info("compressed-tensors: kv_cache_scheme is ignored, the KV cache stays bf16")
+    return W8Config("compressed-tensors", act == ("tensor", False))
+
+
+def _check_ignore(method: str, names):
+    skip = [m for m in names if any(p in m for p in W4_MODULES)]
+    if skip:
+        raise ValueError(f"{method}: the ignore list names quantised projections {skip}")
+
+
+@dataclass
+class W8Tensor:
+    """One W8A8 linear in checkpoint orientation: codes e4m3 [N, K], scale fp32 [N] (per-tensor scales expanded to
+    their rows), input_scale fp32 scalar tensor (static activations) or None."""
+    codes: torch.Tensor
+    scale: torch.Tensor
+    input_scale: Optional[torch.Tensor] = None
+
+
+def fuse_w8(parts, fuse) -> W8Tensor:
+    """The W8Tensor of linears fused into one GEMM: `fuse` applied to their codes and to their scales (each keeps its
+    rows' scale); the static input scale is the largest of theirs."""
+    ins = [p.input_scale for p in parts]
+    return W8Tensor(fuse(*(p.codes for p in parts)), fuse(*(p.scale for p in parts)),
+                    None if ins[0] is None else torch.stack([t.reshape(()) for t in ins]).max())
+
+
+def shard_cols_w8(w: W8Tensor, rank: int, size: int) -> W8Tensor:
+    """Row-parallel shard: this rank's K columns, every output channel's full scale."""
+    return W8Tensor(shard_cols(w.codes, rank, size), w.scale, w.input_scale)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -305,6 +399,29 @@ class CheckpointReader:
             raise ValueError(f"{module}: scales {tuple(scales.shape)} {scales.dtype} / zeros {tuple(zeros.shape)} do "
                              f"not match {cfg.method} codes [{n}, {k}] with group_size {cfg.group_size}")
         return W4Tensor(codes.contiguous(), zeros.t().to(torch.uint8).contiguous(), scales.t().contiguous())
+
+    def get_w8(self, module: str, cfg: W8Config) -> W8Tensor:
+        """`<module>.weight` (+ `.weight_scale`, `.input_scale`) of a W8A8 checkpoint -> `W8Tensor`, codes byte for
+        byte; for `quantization="fp8"` the 16-bit weight quantised per output channel (`ref.fp8_channel_quant`)."""
+        w = self.get_raw(module + ".weight")
+        if cfg.method == "fp8-online":
+            from gllm_b200.ops.ref import fp8_channel_quant
+            return W8Tensor(*fp8_channel_quant(w))
+        if w.dtype != torch.float8_e4m3fn:
+            raise ValueError(f"{module}.weight is {w.dtype}: {cfg.method} W8A8 needs e4m3 weights")
+        n = w.shape[0]
+        s = self.get_raw(module + ".weight_scale")
+        if s.dtype not in (torch.float32, torch.bfloat16, torch.float16) or s.numel() not in (1, n):
+            raise ValueError(f"{module}.weight_scale {tuple(s.shape)} {s.dtype}: expected one fp32 / bf16 scale per "
+                             f"tensor or per output channel ({n})")
+        scale = s.float().reshape(-1).expand(n).contiguous()
+        ins = None
+        if cfg.static:
+            i = self.get_raw(module + ".input_scale")
+            if i.numel() != 1:
+                raise ValueError(f"{module}.input_scale {tuple(i.shape)}: a static activation scale is one scalar")
+            ins = i.float().reshape(())
+        return W8Tensor(w.contiguous(), scale, ins)
 
     def get_rows(self, name: str, start: int, end: int) -> torch.Tensor:
         key = self.resolve(name)

@@ -12,7 +12,7 @@ import torch
 
 from gllm_b200.ops import ref
 from gllm_b200.ops.lib import GemmComm
-from gllm_b200.ops.ref import Int4Weight
+from gllm_b200.ops.ref import Fp8Weight, Int4Weight
 from gllm_b200.ops.ref import (grouped_topk, kv_copy_pages, logprobs_final,  # noqa: F401  (sm100 signatures)
                                logprobs_shard, prompt_logprobs_shard, rope_kv_write, topk_softmax)
 from gllm_b200.parallel import state as ps
@@ -28,6 +28,8 @@ def linear(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None
     assert comm is None and epi == 0, "GEMM epilogues over peer memory are sm_90a only"
     if isinstance(w, Int4Weight):
         return linear_w4a16(x, w, bias, out=out)
+    if isinstance(w, Fp8Weight):
+        return linear_fp8(x, w, bias, out=out)
     if isinstance(w, tuple):
         return linear_fp8_block(x, w[0], w[1], bias, out=out)
     return _into(out, ref.linear(x, w, bias))
@@ -37,6 +39,16 @@ def linear_w4a16(x: torch.Tensor, w: Int4Weight, bias: Optional[torch.Tensor] = 
                  out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """The device layout unpacked and de-quantised to x's dtype (`ref.w4a16_dequant`), then `ref.linear`."""
     return _into(out, ref.linear_w4a16(x, w, bias))
+
+
+def fp8_quant_token(x: torch.Tensor, input_scale: Optional[torch.Tensor] = None):
+    return ref.fp8_quant_token(x, input_scale)
+
+
+def linear_fp8(x: torch.Tensor, w: Fp8Weight, bias: Optional[torch.Tensor] = None,
+               out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Per-token quantised activations times the e4m3 codes, scaled after an fp32 sum (`ref.linear_fp8`)."""
+    return _into(out, ref.linear_fp8(x, w, bias))
 
 
 def linear_silu_mul(x: torch.Tensor, w_interleaved: torch.Tensor, out: Optional[torch.Tensor] = None,

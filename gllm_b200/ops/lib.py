@@ -117,6 +117,9 @@ ABI = {
     "gllm_fp8_quant_group": [P, L, P, P, I, I, P],
     "gllm_moe_grouped_gemm_fp8": [P, P, P, P, P, L, I, I, I, I, P, P, I, P],
     "gllm_gemm_fp8_block": [P, P, P, P, P, L, I, I, I, P, P],
+    "gllm_fp8_quant_token": [P, L, P, P, P, I, I, P],
+    "gllm_gemm_fp8_w8a8": [P, P, P, P, P, L, I, I, I, P, P],
+    "gllm_gemm_fp8_smallm": [P, P, P, P, P, L, I, I, I, P, I, P, L, P, P],
     "gllm_lora_shrink": [P, L, P, P, P, I, I, I, P, P, P, I, I, P],
     "gllm_lora_expand_add": [P, L, P, P, L, I, I, I, I, I, I, P, P, P, I, P],
     "gllm_lora_expand_silu_mul": [P, L, P, L, P, P, L, I, I, I, P, P, P, I, P],

@@ -627,6 +627,56 @@ def linear_fp8_block(x: torch.Tensor, w: torch.Tensor, w_scale_inv: torch.Tensor
     return y.to(x.dtype)
 
 
+class Fp8Weight:
+    """Weight handle of a W8A8 linear (per-channel / per-tensor FP8 checkpoints, `quantization="fp8"`), the same on every
+    device: `codes` e4m3 [N, K] contiguous and `scale` fp32 [N], so that W[n, k] = scale[n] · codes[n, k];
+    `input_scale` a fp32 scalar tensor for static activation scales, None for dynamic per-token ones. Not a tuple: the
+    linear ops send tuples to the block-scaled GEMM."""
+    __slots__ = ("codes", "scale", "input_scale")
+
+    def __init__(self, codes, scale, input_scale=None):
+        self.codes, self.scale, self.input_scale = codes, scale, input_scale
+
+    @property
+    def out_features(self) -> int:
+        return self.codes.shape[0]
+
+
+def fp8_quant_token(x: torch.Tensor, input_scale: Optional[torch.Tensor] = None):
+    """Per-token activation quantisation of the W8A8 path (csrc/gemm/gemm_fp8_block.cu:fp8_quant_token_kernel, bit
+    for bit) -> (e4m3 [M, K], fp32 scales [M]). Dynamic: s = max(amax_k |x|, 1e-10) / 448, q = e4m3_rn(x · (1 / s)),
+    the reciprocal first. Static: s = input_scale, q = e4m3_rn(clamp(x / s, ±448)). Rounding saturates to ±448."""
+    xf = x.float()
+    if input_scale is None:
+        s = xf.abs().amax(-1).clamp_min(1e-10) / FP8_MAX if x.shape[1] else torch.full(
+            (x.shape[0],), 1e-10 / FP8_MAX, device=x.device)
+        v = xf * torch.reciprocal(s).unsqueeze(-1)
+    else:
+        s = input_scale.float().reshape(1).expand(x.shape[0]).clone()
+        v = xf / s.unsqueeze(-1)
+    return v.clamp(-FP8_MAX, FP8_MAX).to(torch.float8_e4m3fn), s
+
+
+def linear_fp8(x: torch.Tensor, w: Fp8Weight, bias: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """W8A8: y = dtype(acc · s_x[m] · s_w[n] + bias[n]) with acc = Σ_k x_q · w_q in fp32. The products of two e4m3
+    values and their sum over K < 2^31 / 448^2 terms are exact in float64, so acc here is the exact sum rounded once:
+    the same for every batch composition."""
+    xq, xs = fp8_quant_token(x, w.input_scale)
+    acc = (xq.double() @ w.codes.double().t()).float()
+    y = acc * xs.unsqueeze(-1) * w.scale.float().unsqueeze(0)
+    if bias is not None:
+        y = y + bias.float()
+    return y.to(x.dtype)
+
+
+def fp8_channel_quant(w: torch.Tensor):
+    """Online quantisation of a 16-bit weight [N, K] -> (e4m3 codes [N, K], fp32 scale [N]):
+    s[n] = max(amax_k |w[n, k]|, 1e-12) / 448, codes = e4m3_rn(w / s)."""
+    wf = w.float()
+    s = wf.abs().amax(-1).clamp_min(1e-12) / FP8_MAX
+    return (wf / s.unsqueeze(-1)).clamp(-FP8_MAX, FP8_MAX).to(torch.float8_e4m3fn), s
+
+
 def merge_attn_states(o1: torch.Tensor, lse1: torch.Tensor, o2: torch.Tensor, lse2: torch.Tensor):
     """LSE-weighted merge of two partial attention results. o [T,H,D], lse [T,H] (natural log)."""
     m = torch.maximum(lse1, lse2)

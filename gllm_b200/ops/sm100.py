@@ -12,7 +12,7 @@ import torch
 
 from gllm_b200.ops import lib as _lib
 from gllm_b200.ops.lib import GemmComm, _p, check, launch, launches, stream_ptr  # noqa: F401 (launches: bench.py)
-from gllm_b200.ops.ref import Int4Weight
+from gllm_b200.ops.ref import Fp8Weight, Int4Weight
 # the MoE front-ends, so that a model module sees one table
 from gllm_b200.ops.sm100_moe import fused_experts, fused_experts_fp8, grouped_topk, topk_softmax  # noqa: F401
 
@@ -52,10 +52,12 @@ def _linear_smallm(x, w, bias, out, silu: bool):
 
 def linear(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None,
            out: Optional[torch.Tensor] = None, comm: Optional[GemmComm] = None, epi: int = 0) -> torch.Tensor:
-    """y = x @ w.T (+ bias). x [M, K] (row stride arbitrary, unit inner stride), w [N, K], (e4m3, scale_inv) or an
-    `Int4Weight`."""
+    """y = x @ w.T (+ bias). x [M, K] (row stride arbitrary, unit inner stride), w [N, K], (e4m3, scale_inv), an
+    `Int4Weight` or an `Fp8Weight`."""
     if isinstance(w, Int4Weight):
         return linear_w4a16(x, w, bias, out=out)
+    if isinstance(w, Fp8Weight):
+        return linear_fp8(x, w, bias, out=out)
     if isinstance(w, tuple):
         return linear_fp8_block(x, w[0], w[1], bias, out=out)
     assert x.dtype == _BF16 and w.dtype == _BF16, (x.dtype, w.dtype)
@@ -531,6 +533,52 @@ def linear_fp8_block(x: torch.Tensor, w8: torch.Tensor, w_scale_inv: torch.Tenso
         return out
     xq, xs = fp8_quant_group(x)
     launch("gllm_gemm_fp8_block", _p(xq), _p(xs), _p(w8), _p(w_scale_inv), _p(out), out.stride(0), m, n, k, _p(bias))
+    return out
+
+
+# ----------------------------------------------------------------------------------------------
+# W8A8: per-channel / per-tensor FP8 weights, per-token FP8 activations
+# ----------------------------------------------------------------------------------------------
+_FP8_E4M3 = torch.float8_e4m3fn
+_FP8_SMALLM_MAX = int(os.environ.get("GLLM_FP8_SMALLM_MAX", "64"))   # M <= this -> swap-AB split-K kernel (<= 128)
+
+
+def fp8_quant_token(x: torch.Tensor, input_scale: Optional[torch.Tensor] = None):
+    """bf16 [M, K] (row stride arbitrary, unit inner stride) -> (e4m3 [M, K] contiguous, fp32 scales [M]): per-token
+    dynamic scales, or the static fp32 scalar `input_scale` (csrc/gemm/gemm_fp8_block.cu, `ref.fp8_quant_token`)."""
+    assert x.dtype == _BF16 and x.dim() == 2 and x.stride(1) == 1
+    assert input_scale is None or (input_scale.dtype == torch.float32 and input_scale.numel() == 1)
+    m, k = x.shape
+    q = torch.empty(m, k, dtype=_FP8_E4M3, device=x.device)
+    s = torch.empty(m, dtype=torch.float32, device=x.device)
+    launch("gllm_fp8_quant_token", _p(x), x.stride(0), _p(q), _p(s), _p(input_scale), m, k)
+    return q, s
+
+
+def linear_fp8(x: torch.Tensor, w: Fp8Weight, bias: Optional[torch.Tensor] = None,
+               out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """y = bf16(acc · s_x[m] · s_w[n] + bias[n]), acc the fp32 sum of x_q · w_q, with x quantised per token first.
+    M <= _FP8_SMALLM_MAX runs the swap-AB split-K kernel (csrc/gemm/gemm_bf16_smallm.cu, partials reduced in a fixed
+    order in the small-M workspace), larger M the persistent wgmma GEMM (csrc/gemm/gemm_fp8_block.cu). K % 16 == 0."""
+    assert isinstance(w, Fp8Weight) and w.codes.dtype == _FP8_E4M3 and w.codes.is_contiguous()
+    assert w.scale.dtype == torch.float32 and w.scale.is_contiguous() and w.scale.numel() == w.codes.shape[0]
+    assert x.dim() == 2 and x.shape[1] == w.codes.shape[1], (x.shape, w.codes.shape)
+    m, k = x.shape
+    n = w.codes.shape[0]
+    if out is None:
+        out = torch.empty(m, n, dtype=_BF16, device=x.device)
+    else:
+        assert out.shape == (m, n) and out.stride(1) == 1 and out.dtype == _BF16
+    if m == 0:
+        return out
+    xq, xs = fp8_quant_token(x, w.input_scale)
+    if m <= _FP8_SMALLM_MAX:
+        ws, cnt, _ = _smallm_workspace(x.device)
+        launch("gllm_gemm_fp8_smallm", _p(xq), _p(xs), _p(w.codes), _p(w.scale), _p(out), out.stride(0), m, n, k,
+               _p(bias), _FORCE_SPLIT, _p(ws), ws.numel(), _p(cnt))
+    else:
+        launch("gllm_gemm_fp8_w8a8", _p(xq), _p(xs), _p(w.codes), _p(w.scale), _p(out), out.stride(0), m, n, k,
+               _p(bias))
     return out
 
 
